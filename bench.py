@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- edges/sec of the RGCN hot path on a PPI-shaped batch (BASELINE.json configs[1]).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path over one batch: graph_num_layers = 3 x sparse_rgcn_layer
@@ -16,7 +16,7 @@ own counter (models/sparse_graph_model.py:285,310: sum of E_l per batch, counted
                calls (the headline e2e); the same calls recorded once into a CUDA graph and replayed are reported
                beside it (graph_replay_value).
   roofline     algorithmic bytes of one RGCN layer (SURVEY.md 8d: M*(4D+12) + V*8D + L*D*D*4) / measured layer
-               time, against the measured HBM copy bandwidth of MEASURED_PEAKS.json.
+               time, against the HBM bandwidth of the H100 SXM data sheet (3.35 TB/s).
   cpu_baseline the torch-CPU restatement of the reference op order (oracle/ref_torch.py) on this box's cores.
   value_uncached_weights   the same step with the weight-image cache OFF (pack_b_kernel inside the timed region): what a
                training step, whose weights change every step, pays.
@@ -27,6 +27,10 @@ own counter (models/sparse_graph_model.py:285,310: sum of E_l per batch, counted
                ms per layer, the exchange kernel alone, halo bytes, parity against the reference-generated fixture.
 Multi-GPU headline: weak scaling, every rank owns its own batch (graphs are independent units: no collective on the
 data path); value = edges of all ranks / max-over-ranks time.  The sharded block is the strong-scaling companion.
+
+--dump-outputs DIR writes what the timed step computed in its last timed step -- the final node states [V, 256] of the
+3-layer stack, as a caller of the step receives them -- to DIR/rgcn_stack_out.npy (float32, rank 0).  The inputs are seeded, so
+two builds run with the same arguments can be compared output for output.
 """
 import argparse
 import json
@@ -71,7 +75,7 @@ def make_inputs(seed):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     QUERY = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
              "clocks_event_reasons.sw_power_cap")
@@ -204,14 +208,21 @@ def cpu_baseline(batch, h0, layer_weights, budget_s=12.0):
 
 
 def load_peaks():
-    """Roofline denominators: the driver-measured numbers of MEASURED_PEAKS.json, else B200_PROFILING.md's fallback."""
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        with open(path) as f:
-            d = json.load(f)
-        return {"hbm": float(d["hbm_gbs"]), "bf16": float(d["bf16_tflops"]), "bf16_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
-                "source": "MEASURED_PEAKS.json (measured copy bandwidth / cuBLAS bf16)"}
-    return {"hbm": 6650.0, "bf16": 1650.0, "bf16_sustained": 1400.0, "source": "fallback of B200_PROFILING.md"}
+    """Roofline denominators: NVIDIA's data sheet for the H100 SXM (a 700 W card; a card at a lower power limit may not reach
+    them -- the card's name and limit are reported beside the results)."""
+    return {"hbm": 3350.0, "tf32": 495.0, "source": "H100 SXM data sheet: 3.35 TB/s HBM3, 495 TFLOP/s dense TF32 (not measured)"}
+
+
+def gpu_info(index):
+    """Name and power limit of the card the numbers were measured on."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power, clock = [x.strip() for x in out.split(",")]
+        return {"name": name, "power_limit_w": float(power), "max_sm_mhz": float(clock)}
+    except Exception:
+        import torch
+        return {"name": torch.cuda.get_device_name(index), "power_limit_w": None, "max_sm_mhz": None}
 
 
 def time_graph(fn, dev, flush, n=20, warmup=3):
@@ -251,7 +262,8 @@ def extra_configs(dev, flush, peaks):
     import tf_gnn_samples_b200 as G
     from tf_gnn_samples_b200 import batching, weights as W
     hbm = peaks["hbm"]
-    tensor_peak = peaks["bf16_sustained"] / 2.0 / 3.0        # TF32 rate = bf16 / 2; fp32-accurate products need 3 TF32 passes
+    tensor_peak = peaks["tf32"] / 3.0                          # fp32-accurate products need 3 TF32 passes
+    gpu = "1x" + torch.cuda.get_device_name(dev)
     lines = []
 
     def states(V, D):
@@ -266,12 +278,12 @@ def extra_configs(dev, flush, peaks):
     w = W.to_torch(W.ggnn_weights(L, D), dev)
     ms = time_graph(lambda: G.sparse_ggnn_layer(h, plan, D, num_timesteps=T, weights=w), dev, flush)
     flops = T * (V * L * D * D * 2 + V * (2 * D) * (3 * D) * 2)          # SURVEY 8d: 59 GF per timestep
-    lines.append({"config": "config 3: GGNN QM9 10k graphs (real validation molecules: V=%d M=%d L=%d) hidden=128 GRU %d timesteps, 1xB200" % (V, M, L, T),
+    lines.append({"config": "config 3: GGNN QM9 10k graphs (real validation molecules: V=%d M=%d L=%d) hidden=128 GRU %d timesteps, %s" % (V, M, L, T, gpu),
                   "ms_per_call": ms, "ms_per_timestep": ms / T, "edges_per_s": M / (ms * 1e-3),
                   "roofline": {"bound": "tensor", "achieved": flops / (ms * 1e-3) / 1e12, "peak": tensor_peak, "unit": "TFLOP/s",
                                "frac": flops / (ms * 1e-3) / 1e12 / tensor_peak,
                                "what": "algorithmic fp32 FLOPs (SURVEY.md 8d: per timestep V*L*D^2*2 for the per-type transforms + V*2D*3D*2 for the GRU) / time, "
-                                       "against the fp32-accurate tensor peak = measured sustained bf16 / 2 (TF32 rate) / 3 (3xTF32 split products)",
+                                       "against the fp32-accurate tensor peak = data-sheet dense TF32 / 3 (3xTF32 split products)",
                                "hbm_frac_of_algorithmic_bytes": T * (M * (4 * D + 8) + V * 8 * D + L * D * D * 4) / (ms * 1e-3) / 1e9 / hbm}})
     plan.close()
     # ---- config 4: RGAT on the PPI-shaped batch, hidden 256, 8 heads ----
@@ -282,7 +294,7 @@ def extra_configs(dev, flush, peaks):
     w = W.to_torch(W.rgat_weights(L, D, D), dev)
     ms = time_graph(lambda: G.sparse_rgat_layer(h, plan, D, num_heads=K, activation_function="tanh", weights=w), dev, flush)
     alg = M * (4 * D + 8 + 4 * K) + V * 8 * D + L * D * D * 4
-    lines.append({"config": "config 4: RGAT PPI-shaped (V=%d M=%d L=%d) hidden=256 8 heads, 1xB200" % (V, M, L), "ms_per_call": ms,
+    lines.append({"config": "config 4: RGAT PPI-shaped (V=%d M=%d L=%d) hidden=256 8 heads, %s" % (V, M, L, gpu), "ms_per_call": ms,
                   "edges_per_s": M / (ms * 1e-3),
                   "roofline": {"bound": "hbm", "achieved": alg / (ms * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s", "frac": alg / (ms * 1e-3) / 1e9 / hbm,
                                "what": "algorithmic bytes M*(4D + 8 + 4K) + V*8D + L*D^2*4 (SURVEY.md 8d) / time"}})
@@ -297,7 +309,7 @@ def extra_configs(dev, flush, peaks):
     ms = time_graph(lambda: G.sparse_gnn_film_layer(h, plan, cnt, D, weights=w), dev, flush)
     alg = M * (4 * D + 8) + V * 8 * D + L * D * D * 4 + V * L * 8 * D
     flops = V * L * D * D * 2 * 3                                          # W_l h (D) + F_l h (2D) per (node, type)
-    lines.append({"config": "config 5 on one GPU: GNN-FiLM VarMisuse-shaped random graph (V=%d M=%d L=%d) hidden=128, 1xB200" % (V, M, L),
+    lines.append({"config": "config 5 on one GPU: GNN-FiLM VarMisuse-shaped random graph (V=%d M=%d L=%d) hidden=128, %s" % (V, M, L, gpu),
                   "ms_per_call": ms, "edges_per_s": M / (ms * 1e-3),
                   "roofline": {"bound": "hbm", "achieved": alg / (ms * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s", "frac": alg / (ms * 1e-3) / 1e9 / hbm,
                                "what": "algorithmic bytes M*(4D + 8) + V*8D + L*D^2*4 + gamma/beta rows V*L*8D (SURVEY.md 8d) / time",
@@ -477,7 +489,7 @@ def run_ours(args, rank, world, local_rank):
     torch.cuda.synchronize()
     assert torch.equal(out_graph, out_eager), "CUDA-graph replay differs from eager execution"
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > the 50 MB L2
 
     def timed_steps(fn, steps, warmup):
         for _ in range(warmup):
@@ -503,6 +515,7 @@ def run_ours(args, rank, world, local_rank):
     if sampler:
         sampler.start()
     total_ms, per_step = timed_steps(graph.replay, args.steps, args.warmup)
+    dumped = out_graph.cpu() if args.dump_outputs else None   # the last timed step's result, before anything else runs
     # roofline leg: ONE layer (transform GEMM + edge-stage segment kernel) as its own CUDA graph, same cold-L2
     # protocol -- the kernels' device time without host launch latency between them
     def one_layer():
@@ -549,6 +562,9 @@ def run_ours(args, rank, world, local_rank):
     uncached_total_ms, _ = timed_steps(graph_uncached.replay, args.steps, args.warmup)
     G.set_weight_cache(True)
     clocks = sampler.stop() if sampler else None
+    if dumped is not None and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "rgcn_stack_out.npy"), dumped.numpy().astype(np.float32))
 
     total_ms = max_over_ranks(total_ms)
     ms_per_step = total_ms / args.steps
@@ -598,8 +614,7 @@ def run_ours(args, rank, world, local_rank):
         copy_stream.wait_stream(main)                         # keeps the DMA order: structure, then features
         with torch.cuda.stream(copy_stream):
             stage_dev[off_h:].copy_(stage_host[off_h:], non_blocking=True)
-            # One device-side copy out of the DMA landing buffer: kernels reading the landing buffer directly ran
-            # 3-4x slower on this platform (tools/e2e_probe.py: plan 341 vs 82 us, layers 382 vs 135 us).
+            # One device-side copy out of the DMA landing buffer: the kernels read the copy, not the landing buffer.
             work_h = stage_dev[off_h:].clone()
         work_g = stage_dev[:off_h].clone()
         cd = dev_view(work_g, "cnt")
@@ -690,15 +705,6 @@ def run_ours(args, rank, world, local_rank):
     # step time / layers (cold L2 for the first layer of every step, the later layers start from what the previous one left)
     layer_in_step_ms = ms_per_step / NUM_LAYERS
     achieved = layer_bytes / (layer_in_step_ms * 1e-3) / 1e9
-    traffic = None
-    traffic_src = None
-    for name in ("r02_traffic.json", "r01_traffic.json"):      # written from the round's own ncu --set full capture (tools/ncu_traffic.py)
-        tpath = os.path.join(ROOT, "profiles", name)
-        if os.path.exists(tpath):
-            with open(tpath) as f:
-                traffic = json.load(f).get("dram_bytes_per_layer")
-            traffic_src = "profiles/" + name
-            break
     line = {
         "metric": METRIC, "value": value, "unit": "edges/s", "n_gpus": world, "steps": args.steps,
         "warmup": args.warmup, "ms_per_step": ms_per_step, "higher_is_better": True, "scaling": "weak",
@@ -709,19 +715,19 @@ def run_ours(args, rank, world, local_rank):
                     "parallelism": "independent batch per rank (graph-boundary sharding, no collective); see 'sharded' for the node-range-sharded single graph",
                     "weights": "value: static weights, packed TF32 hi/lo weight images cached across steps (rgnn_set_weight_cache); "
                                "value_uncached_weights: cache off, pack_b_kernel inside the timed region",
-                    "warm_l2_ms_per_step": warm_ms, "per_layer_edges_per_s": M / (layer_ms * 1e-3)},
+                    "warm_l2_ms_per_step": warm_ms, "per_layer_edges_per_s": M / (layer_ms * 1e-3),
+                    "gpu": gpu_info(local_rank)},
         "value_uncached_weights": {"value": edges_all / (uncached_ms * 1e-3), "unit": "edges/s", "ms_per_step": uncached_ms,
                                    "kernels_per_step": int(kernels_uncached),
                                    "roofline_frac": layer_bytes / (uncached_ms / NUM_LAYERS * 1e-3) / 1e9 / peak},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src, "kernel": "one RGCN layer = gemm_tcgen05_kernel (node transform, tcgen05 3xTF32) + seg_reduce_kernel (fused edge stage)",
+                     "kernel": "one RGCN layer = gemm_wgmma_kernel (node transform, wgmma 3xTF32) + seg_reduce_kernel (fused edge stage)",
                      "algorithmic_bytes_per_launch": layer_bytes, "ms_per_launch": layer_in_step_ms,
                      "ms_per_launch_what": "timed region / (steps x layers): average duration of one layer inside the step",
                      "ms_single_layer_cold_l2": layer_ms, "frac_single_layer_cold_l2": layer_bytes / (layer_ms * 1e-3) / 1e9 / peak,
                      "ms_single_layer_via_python_api": layer_api_ms, "peak_source": peak_src,
-                     "note": "working set is L2-resident: DRAM traffic (ncu) is 11.8 MB per layer vs 130 MB algorithmic, so frac "
-                             "compares algorithmic bytes with the HBM copy peak; the binding resource is L2->SM delivery "
-                             "(165 MB per layer at ~7 TB/s), see DESIGN.md 5.3 and profiles/r01_final_kernels.txt"},
+                     "note": "the layer's working set (inputs, plan, weights: ~10 MB) fits the 50 MB L2, so the algorithmic bytes "
+                             "are not all HBM traffic: frac compares them with the HBM peak"},
         "e2e": {"value": e2e_value, "unit": "edges/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                 "ms_per_step": e2e_eager_s / args.steps * 1e3, "mode": "eager public-API calls every step (GraphPlan + rgcn_layer_stack)",
                 "graph_replay_value": e2e_graph_value,
@@ -762,6 +768,8 @@ def main():
     ap.add_argument("--skip-e2e", action="store_true", help="profiling runs: leave out the host-buffer leg")
     ap.add_argument("--skip-configs", action="store_true", help="leave out the lines for BASELINE configs 3-5")
     ap.add_argument("--skip-sharded", action="store_true", help="N > 1: leave out the node-range-sharded config-5 block")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's result to DIR/rgcn_stack_out.npy (float32)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     rank = int(os.environ.get("RANK", "0"))

@@ -1,5 +1,5 @@
 /*
- * rgnn.h -- C ABI of the B200-native relational message-passing engine (librgnn.so).
+ * rgnn.h -- C ABI of the H100-native relational message-passing engine (librgnn.so).
  *
  * The reference (microsoft/tf-gnn-samples) has no FFI: its boundary is the Python call
  * convention  Sparse_Graph_Model._apply_gnn_layer(node_representations, adjacency_lists,

@@ -1,7 +1,7 @@
 """Writes tests/golden/ref_batcher_feeds.npz by running the REFERENCE's own loaders and batchers (tasks/qm9_task.py,
 tasks/ppi_task.py, unmodified, under tests/tf1_shim -- only tf.placeholder as a dict key and dpu_utils RichPath are involved):
 
-    python tests/golden/make_batcher_fixtures.py            (needs /root/reference; not available on the GPU box)
+    python tests/golden/make_batcher_fixtures.py            (needs the original checkout: TF_GNN_SAMPLES_REFERENCE=<path>)
 
 QM9 cases run on the 200 real validation molecules of qm9_valid_subset.json.gz, PPI cases on a seeded fold in the dgl file
 layout (batcher_cases.write_ppi_dir).  Every minibatch feed of every case is stored (keys <case>/b<i>/<placeholder name>);

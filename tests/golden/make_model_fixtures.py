@@ -1,7 +1,7 @@
 """Writes tests/golden/ref_model_<case>.npz by running the REFERENCE's own model scaffold and task heads (models/*.py,
 tasks/{ppi,qm9}_task.py, unmodified, built eagerly under tests/tf1_shim.graph_mode; see model_cases.py):
 
-    python tests/golden/make_model_fixtures.py [case ...]          (needs /root/reference; not available on the GPU box)
+    python tests/golden/make_model_fixtures.py [case ...]          (needs the original checkout: TF_GNN_SAMPLES_REFERENCE=<path>)
 
 Per case: the pickle the reference's own save_model wrote (weights under the reference's variable names + params), the
 final node representations and task metrics of the float64 run, the float32 run's error against it (err32), and the

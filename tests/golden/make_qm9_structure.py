@@ -1,7 +1,7 @@
 """Regenerates tests/golden/qm9_valid_structure.npz: the GRAPH STRUCTURE (atoms per molecule, bonds as (src, type, dst)) of all
 10,000 records of the reference's data/qm9/valid.jsonl.gz -- BASELINE config 3 ("GGNN QM9, 10k-graph batch") on the real
 molecules rather than a shape-matched synthetic batch.  Node features and targets are not included (the 200-record subset
-in qm9_valid_subset.json.gz carries those for the parity tests).  Needs /root/reference (this container only)."""
+in qm9_valid_subset.json.gz carries those for the parity tests).  Needs the original checkout (TF_GNN_SAMPLES_REFERENCE)."""
 import os
 import sys
 

@@ -1,5 +1,5 @@
 """Regenerates tests/golden/qm9_valid_subset.json.gz: the first 200 records of the reference's data/qm9/valid.jsonl.gz
-(graph triples, 15-d node features, 13 targets), re-serialised compactly.  Needs /root/reference (this container only);
+(graph triples, 15-d node features, 13 targets), re-serialised compactly.  Needs the original checkout (TF_GNN_SAMPLES_REFERENCE);
 the committed subset is what the tests read on the GPU box."""
 import gzip
 import json

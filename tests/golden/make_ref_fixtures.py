@@ -1,6 +1,6 @@
 """Generates tests/golden/ref_*.npz by EXECUTING THE REFERENCE'S OWN LAYER CODE.
 
-    python tests/golden/make_ref_fixtures.py [case ...]         (needs /root/reference; not available on the GPU box)
+    python tests/golden/make_ref_fixtures.py [case ...]         (needs the original checkout: TF_GNN_SAMPLES_REFERENCE=<path>)
 
 The unmodified ``/root/reference/gnns/*.py`` + ``utils/utils.py`` are imported with tests/tf1_shim standing in for
 ``tensorflow`` / ``dpu_utils`` (numpy-backed, eager: only the TF kernel semantics are restated, see the shim's docstring),
@@ -75,8 +75,7 @@ def make_case(name):
     blob.update(input_checksums(h, adj, indeg))
     if case.get("big"):
         blob.update(RC.summarize(out64))
-        s32 = RC.summarize(out32)
-        blob["out32_rows"] = s32["out_rows"].astype(np.float32)
+        blob["out32_rows"] = out32[blob["rows"]].astype(np.float32)
     else:
         blob.update({"h": h, "indeg": indeg, "out": out64, "out32": out32})
         for l, a in enumerate(adj):

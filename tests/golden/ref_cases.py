@@ -148,12 +148,31 @@ def projection_vector(dim):
     return np.random.default_rng(PROJECTION_SEED).standard_normal(dim)
 
 
+MAX_SUMMARY_ROWS = 256     # keeps every committed file under 1 MB: larger outputs commit every k-th of the stride-97 rows
+PROJ_BLOCK_ABOVE = 20000   # ... and, above this many rows, the projection summed over blocks of PROJ_BLOCK rows
+PROJ_BLOCK = 16
+
+
 def summarize(out64):
     """What a big case commits of a [V, D] float64 output."""
     out64 = np.asarray(out64, np.float64)
-    return {"rows": np.arange(0, out64.shape[0], BIG_ROW_STRIDE), "out_rows": out64[::BIG_ROW_STRIDE].copy(),
-            "proj": out64 @ projection_vector(out64.shape[1]), "colsum": out64.sum(axis=0),
-            "maxabs": np.float64(np.abs(out64).max()), "shape": np.asarray(out64.shape)}
+    return compact_summary({"rows": np.arange(0, out64.shape[0], BIG_ROW_STRIDE), "out_rows": out64[::BIG_ROW_STRIDE].copy(),
+                            "proj": out64 @ projection_vector(out64.shape[1]), "colsum": out64.sum(axis=0),
+                            "maxabs": np.float64(np.abs(out64).max()), "shape": np.asarray(out64.shape)})
+
+
+def compact_summary(blob):
+    """Thin the committed rows to at most MAX_SUMMARY_ROWS and block-sum the projection of large outputs (out32_rows, when
+    present, follows the rows)."""
+    blob = dict(blob)
+    k = -(-len(blob["rows"]) // MAX_SUMMARY_ROWS)
+    for key in ("rows", "out_rows", "out32_rows"):
+        if key in blob:
+            blob[key] = np.ascontiguousarray(blob[key][::k])
+    if int(blob["shape"][0]) > PROJ_BLOCK_ABOVE and "proj_block" not in blob:
+        blob["proj"] = np.add.reduceat(blob["proj"], np.arange(0, len(blob["proj"]), PROJ_BLOCK))
+        blob["proj_block"] = np.int64(PROJ_BLOCK)
+    return blob
 
 
 def compare_with_summary(got, z, what=""):
@@ -166,7 +185,10 @@ def compare_with_summary(got, z, what=""):
     assert tuple(got.shape) == tuple(int(x) for x in z["shape"]), "%s: shape %s vs %s" % (what, got.shape, z["shape"])
     scale = float(z["maxabs"])
     r = projection_vector(got.shape[1])
-    err_rows = float(np.abs(got[::BIG_ROW_STRIDE] - z["out_rows"]).max() / scale)
-    err_proj = float(np.abs(got @ r - z["proj"]).max() / (scale * np.abs(r).sum()))
+    err_rows = float(np.abs(got[z["rows"]] - z["out_rows"]).max() / scale)
+    proj, block = got @ r, int(z["proj_block"]) if "proj_block" in z else 1
+    if block > 1:                                          # a sum of `block` row projections: error bound grows by `block`
+        proj = np.add.reduceat(proj, np.arange(0, len(proj), block))
+    err_proj = float(np.abs(proj - z["proj"]).max() / (scale * np.abs(r).sum() * block))
     err_col = float(np.abs(got.sum(axis=0) - z["colsum"]).max() / (scale * got.shape[0]))
     return err_rows, err_proj, err_col

@@ -37,7 +37,7 @@ def test_timed_port_equals_the_reference_at_config_2():
     bound = 4 * float(z["err32"]) + 1e-6
     assert max(err_rows, err_proj, err_col) <= bound, (err_rows, err_proj, err_col, bound)
     scale = float(z["maxabs"])
-    assert np.abs(out[::RC.BIG_ROW_STRIDE].astype(np.float64) - z["out32_rows"].astype(np.float64)).max() / scale <= 2e-6
+    assert np.abs(out[z["rows"]].astype(np.float64) - z["out32_rows"].astype(np.float64)).max() / scale <= 2e-6
 
 
 def test_the_three_layer_stack_bench_times_is_the_oracles():

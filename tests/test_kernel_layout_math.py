@@ -1,5 +1,5 @@
 """CPU: the index arithmetic the tensor-core kernels rely on, replayed in numpy -- shared-memory operand images
-(K-major, 128-byte swizzle), the lane maps of the producers (forward GEMM, transposing TN GEMM) and of the epilogue staging.
+(K-major, 128-byte swizzle), the lane maps of the producers (forward GEMM, transposing TN GEMM) and of the wgmma accumulator.
 Each test states the property the kernel comment claims (every element written exactly once; no shared-memory bank
 conflicts inside a quarter-warp of a 128-bit access; coalesced 128-byte global segments) and checks it for all lanes."""
 import numpy as np
@@ -7,7 +7,7 @@ import numpy as np
 
 def sw128_offset(row, chunk16):
     """Byte offset of the 16-byte chunk `chunk16` (4 fp32 of K) of image row `row`: rows are 128 B, the chunk index is
-    XORed with row % 8 (SWIZZLE_128B) -- gemm_tcgen05.cu / gemm_tn_tcgen05.cu / pack_b_kernel."""
+    XORed with row % 8 (SWIZZLE_128B) -- gemm_wgmma.cu / gemm_tn_wgmma.cu / pack_b_kernel."""
     return row * 128 + ((chunk16 ^ (row & 7)) << 4)
 
 
@@ -16,7 +16,7 @@ def bank_groups_16B(byte_offsets):
 
 
 def test_forward_producer_covers_the_tile_once_and_stores_without_conflicts():
-    """gemm_tcgen05_kernel A producers: f = ptid + i*128, row = f >> 3, c16 = f & 7 (i < 8, ptid < 128)."""
+    """gemm_wgmma_kernel A producers: f = ptid + i*128, row = f >> 3, c16 = f & 7 (i < 8, ptid < 128)."""
     seen = np.zeros((128, 8), dtype=int)
     for i in range(8):
         for warp in range(4):
@@ -38,7 +38,7 @@ def test_forward_producer_covers_the_tile_once_and_stores_without_conflicts():
 
 
 def test_transposing_producer_of_the_tn_gemm():
-    """gemm_tn_tcgen05_kernel: lane = l0 | c4 << 1 | gh << 3; image row (= matrix column) 32 w + 4 (l0 + 2 gh) + j;
+    """gemm_tn_wgmma_kernel: lane = l0 | c4 << 1 | gh << 3; image row (= matrix column) 32 w + 4 (l0 + 2 gh) + j;
     16-byte K chunk 4 h + c4; loads A[k0 + 16 h + 4 c4 + i][col .. col + 3]."""
     seen = np.zeros((128, 8), dtype=int)                  # image rows x 16-byte chunks of one 32-wide K step
     for w in range(4):
@@ -78,7 +78,7 @@ def test_packed_weight_image_matches_the_operand_layout():
 
 
 def test_umma_k_step_advance_stays_inside_the_swizzle_atom():
-    """The MMA issuer advances the descriptor start address by 32 bytes per UMMA_K = 8 tf32 (4 steps per 128-byte row):
+    """The consumers advance the descriptor start address by 32 bytes per wgmma K = 8 tf32 (4 steps per 128-byte row):
     element (row, k) of k-step s must be found at base(s) + the swizzled position of (row, k - 8 s) computed with the
     address bits the hardware XORs (bits 4-6 with bits 7-9 of the absolute offset)."""
     def hw_address(base, row, kk):                        # 128B swizzle applied by the hardware on the absolute smem offset
@@ -91,17 +91,19 @@ def test_umma_k_step_advance_stays_inside_the_swizzle_atom():
                 assert hw_address(32 * s, row, kk) == want
 
 
-def test_epilogue_staging_pitch_is_conflict_free_for_writes_and_reads():
-    """EPI_PITCH = 144 B: a lane writes its row (16-byte pieces), later 8 lanes read one row's 128 contiguous bytes."""
-    pitch = 144
-    for qd in range(8):                                   # write phase: lane = row, same 16-byte piece index for all lanes
-        offs = np.array([lane * pitch + qd * 16 for lane in range(32)])
-        for q in range(4):
-            assert len(set(bank_groups_16B(offs[q * 8:(q + 1) * 8]))) == 8
-    for j in range(8):                                    # read phase: sub_row = lane >> 3, sub_c4 = lane & 7
-        offs = np.array([(j * 4 + (lane >> 3)) * pitch + (lane & 7) * 16 for lane in range(32)])
-        for q in range(4):
-            assert len(set(bank_groups_16B(offs[q * 8:(q + 1) * 8]))) == 8
+def test_wgmma_accumulator_fragments_cover_the_tile_once():
+    """epilogue_regs / the TN epilogue: thread t of a consumer warpgroup holds d[4 j + 2 i + e] of row 16 (t / 32) + (t % 32) / 4
+    + 8 i and column 8 j + 2 (t % 4) + e -- every element of the 64 x BN accumulator exactly once, column pairs even-aligned."""
+    for BN in (32, 64, 128):
+        seen = np.zeros((64, BN), dtype=int)
+        for t in range(128):
+            for j in range(BN // 8):
+                for i in range(2):
+                    row, col = 16 * (t // 32) + (t % 32) // 4 + 8 * i, 8 * j + 2 * (t % 4)
+                    assert col % 2 == 0
+                    seen[row, col] += 1
+                    seen[row, col + 1] += 1
+        assert np.all(seen == 1)
 
 
 def test_split_tf32_is_exact_and_three_products_recover_fp32_accuracy():
@@ -131,28 +133,14 @@ def packed_image_offset(BN, nl, c16):
     return ((nl >> 3) * 256 + (nl & 7) * 32 + ((c16 ^ (nl & 7)) << 2)) * 4
 
 
-def test_cta_pair_weight_halves_are_contiguous_swizzle_atoms():
-    """gemm_tcgen05_kernel<PAIR>: CTA r bulk-copies bytes [r * BN/2 * 128, +BN/2 * 128) of the hi image and of the lo image into
-    ITS stage.  For that to be a valid K-major SWIZZLE_128B operand of BN/2 rows the half must (a) hold exactly the rows
-    [r BN/2, (r+1) BN/2) and nothing else, and (b) keep every row's swizzle phase (row & 7) -- i.e. start on an 8-row atom."""
-    for BN in range(32, 257, 32):
-        half_rows, half_bytes = BN // 2, (BN // 2) * 128
-        assert half_rows % 8 == 0                                   # whole 8-row / 1024-byte swizzle atoms (SBO = 1024)
-        for r in (0, 1):
-            for nl in range(r * half_rows, (r + 1) * half_rows):
-                for c16 in range(8):
-                    off = packed_image_offset(BN, nl, c16)
-                    assert r * half_bytes <= off < (r + 1) * half_bytes           # (a) the row lives in this CTA's byte range
-                    local = off - r * half_bytes                                 # where it lands in the CTA's own image
-                    ln = nl - r * half_rows                                      # its row index in the half-height operand
-                    assert local == sw128_offset(ln, c16)                        # (b) same layout as a BN/2-row image built directly
-
-
-def test_pair_mode_shrinks_the_stage_so_that_a_third_ring_stage_fits():
-    ring_budget = 227 * 1024 - 1024 - 18432 - 512                   # TC_RING_BUDGET of gemm_tcgen05.cu
-    stage = lambda bn, pair: 2 * 128 * 128 + 2 * (bn // 2 if pair else bn) * 128   # noqa: E731
-    assert min(4, ring_budget // stage(256, False)) == 2 and min(4, ring_budget // stage(256, True)) == 3
-    assert min(4, ring_budget // stage(128, False)) == 3 and min(4, ring_budget // stage(128, True)) == 4
+def test_ring_stages_fit_the_shared_memory_of_an_sm90_block():
+    """gemm_wgmma.cu: a stage holds the hi and lo images of A (128 rows) and of B (BN rows), 128 B per row; the ring takes what
+    fits into 227 KB of opt-in shared memory less alignment slack and barriers, at most 4 stages -- and never fewer than the
+    2 producer groups (test_producer_groups_never_exceed_ring_stages)."""
+    ring_budget = 227 * 1024 - 1024 - 256                           # TC_RING_BUDGET
+    stage = lambda bn: 2 * 128 * 128 + 2 * bn * 128                 # noqa: E731
+    assert [min(4, ring_budget // stage(bn)) for bn in (32, 64, 128)] == [4, 4, 3]
+    assert 3 * stage(128) + 1024 + 2 * 3 * 8 <= 227 * 1024
 
 
 def test_producer_groups_never_exceed_ring_stages():

@@ -1,4 +1,4 @@
-"""GPU: the exported building blocks against numpy (float64): tcgen05 3xTF32 Dense at awkward shapes,
+"""GPU: the exported building blocks against numpy (float64): wgmma 3xTF32 Dense at awkward shapes,
 segment aggregation in all four modes, layer norm."""
 import numpy as np
 import pytest
@@ -43,7 +43,7 @@ def test_dense_bias_activation(cuda_device):
 @pytest.mark.parametrize("m,k,n", [(1, 4, 4), (31, 8, 12), (33, 132, 260), (2245, 256, 768), (11225, 256, 256),
                                    (5000, 52, 124), (70000, 128, 128), (97, 512, 36)])
 def test_dense_backward_matches_fp64(cuda_device, m, k, n):
-    """grad_x = g . W^T (transposed-weight tcgen05 GEMM) and grad_W = x^T . g (split-K TN kernel) against float64."""
+    """grad_x = g . W^T (transposed-weight wgmma GEMM) and grad_W = x^T . g (split-K TN kernel) against float64."""
     import torch
     rng = np.random.default_rng(m + 3 * k + n)
     x = rng.standard_normal((m, k)).astype(np.float32)
@@ -128,26 +128,3 @@ def test_restricted_target_rows_sharded_execution(cuda_device):
     with pytest.raises(RgnnError):
         own.set_num_targets(part.n_local + 1)
 
-
-def test_cta_pair_gemm_in_a_subprocess(cuda_device):
-    """The tcgen05 cta_group::2 variant of the GEMM (RGNN_GEMM_PAIR=1 is read once per process): dense contractions with
-    bias / activation, ragged M and N, two K segments' worth of chunks -- against float64, same 1e-5 bar as the default path."""
-    import os, subprocess, sys, textwrap
-    code = textwrap.dedent("""
-        import numpy as np, torch, sys
-        sys.path.insert(0, %r)
-        from tf_gnn_samples_b200 import ops
-        from oracle import ref_layers as R
-        rng = np.random.default_rng(0)
-        for (m, k, n) in [(1000, 128, 256), (4097, 256, 384), (300, 64, 96), (129, 32, 32)]:
-            x = rng.standard_normal((m, k)).astype(np.float32); w = (rng.standard_normal((k, n)) / np.sqrt(k)).astype(np.float32)
-            b = rng.standard_normal(n).astype(np.float32)
-            got = ops.dense(torch.as_tensor(x).cuda(), torch.as_tensor(w).cuda(), torch.as_tensor(b).cuda(), "tanh").cpu().numpy()
-            want = np.tanh(x.astype(np.float64) @ w.astype(np.float64) + b)
-            err = R.max_norm_rel_err(got, want)
-            assert err <= 1e-5, (m, k, n, err)
-        print("PAIR_OK")
-    """ % os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-    env = dict(os.environ, RGNN_GEMM_PAIR="1")
-    res = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300)
-    assert "PAIR_OK" in res.stdout, res.stdout + res.stderr

@@ -1,12 +1,9 @@
 """The oracle is pinned against THE REFERENCE'S OWN CODE: tests/golden/ref_*.npz hold outputs of the unmodified
-/root/reference/gnns/*.py + utils/utils.py executed through tests/tf1_shim (tests/golden/make_ref_fixtures.py).
+reference gnns/*.py + utils/utils.py executed through tests/tf1_shim (tests/golden/make_ref_fixtures.py).
 
   test_oracle_matches_reference_fixture      oracle float64 == reference-through-shim float64 to 1e-12 (small cases: every
                                              element; BASELINE configs 2-5: committed rows + projection + column sums), and
                                              the oracle's float32 mode tracks the reference's float32 arithmetic;
-  test_reference_code_reproduces_fixtures    (only where /root/reference exists, i.e. in the build container) re-executes the
-                                             reference through the shim and checks the committed files and the oracle against
-                                             it element by element -- so the fixtures cannot drift from the reference;
   test_variable_names_round_trip             the variables the reference creates, sorted by checkpoint.sort_variables, feed the
                                              oracle and reproduce the same output (pins the TF-name mapping both ways);
   test_engine_matches_reference_fixture      -m gpu: the CUDA engine through the C ABI against the same fixtures at 1e-4, and
@@ -28,7 +25,6 @@ import ref_cases as RC                       # noqa: E402
 from oracle import ref_layers as R           # noqa: E402
 from helpers import assert_parity            # noqa: E402
 
-HAVE_REFERENCE = os.path.isdir("/root/reference/gnns")
 SMALL = [n for n, c in RC.CASES.items() if not c.get("big")]
 BIG = [n for n, c in RC.CASES.items() if c.get("big")]
 # the heavy float64 oracle passes (QM9-10k x 4 timesteps, 1M-edge FiLM) take tens of seconds each: CPU suite runs them once
@@ -76,26 +72,6 @@ def test_oracle_matches_reference_fixture_baseline_configs(name):
     o64 = oracle_run(case, h, adj, indeg, case["weights"](), np.float64)
     err_rows, err_proj, err_col = RC.compare_with_summary(o64, z, name)
     assert max(err_rows, err_proj, err_col) <= 1e-12, (err_rows, err_proj, err_col)
-
-
-@pytest.mark.skipif(not HAVE_REFERENCE, reason="/root/reference is only present in the build container")
-@pytest.mark.parametrize("name", SMALL + ["config2_rgcn_ppi", "config4_rgat_ppi"])
-def test_reference_code_reproduces_fixtures(name):
-    import warnings
-    import make_ref_fixtures as MRF
-    case, z = RC.CASES[name], load(name)
-    h, adj, indeg = case["graph"]()
-    w = case["weights"]()
-    with warnings.catch_warnings():
-        warnings.simplefilter("ignore")       # the reference's docstrings hold '\e' escapes (SyntaxWarning on 3.12)
-        out64, created = MRF.run_reference(case, h, adj, indeg, w, np.float64)
-    assert sorted(created) == [str(s) for s in z["variable_names"]]
-    o64 = oracle_run(case, h, adj, indeg, w, np.float64)
-    assert R.max_norm_rel_err(o64, out64) <= 1e-12              # every element, also for the BASELINE-sized cases
-    if case.get("big"):
-        assert max(RC.compare_with_summary(out64, z, name)) <= 1e-13
-    else:
-        np.testing.assert_allclose(out64, z["out"], rtol=0, atol=1e-13)
 
 
 @pytest.mark.parametrize("name", SMALL)

@@ -6,7 +6,8 @@ PPI fold, train + valid), its batcher makes the minibatches, ``sess.run`` is SCR
 metric dictionary per batch and records the feed_dict the loop assembled), the clock is a counter.  training.train gets the
 same data through batching.py, a stub model producing the same scripted metrics and the same clock -- and must write the
 same log, line for line: epoch headers, Train / Valid lines with loss, MAE / error ratios or micro-F1, graphs / nodes /
-edges per second, save-best lines, early stopping after ``patience`` epochs, the final summary.  Needs /root/reference."""
+edges per second, save-best lines, early stopping after ``patience`` epochs, the final summary.  What the reference's loop
+wrote and fed is recorded in tests/golden/ref_training_loops.json (make_training_fixtures.py runs it)."""
 import gzip
 import importlib
 import json
@@ -15,7 +16,6 @@ import sys
 import types
 
 import numpy as np
-import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 for p in (HERE, os.path.join(HERE, "golden")):
@@ -24,11 +24,15 @@ for p in (HERE, os.path.join(HERE, "golden")):
 
 import batcher_cases as BC      # noqa: E402
 
-pytestmark = pytest.mark.skipif(not os.path.isdir("/root/reference/models"), reason="the reference checkout is not on this box")
 batching = importlib.import_module("tf_gnn_samples_b200.batching")
 training = importlib.import_module("tf_gnn_samples_b200.training")
 
 PATIENCE, MAX_NODES, SEED = 2, 700, 4
+RECORD = os.path.join(HERE, "golden", "ref_training_loops.json")
+QM9_LOOP = dict(task_name="qm9", task_params={"task_ids": [0, 4]},
+                model_params={"hidden_size": 16, "graph_num_layers": 1, "max_nodes_in_batch": MAX_NODES, "patience": PATIENCE, "random_seed": SEED})
+PPI_LOOP = dict(task_name="ppi", task_params={}, max_nodes=120,
+                model_params={"hidden_size": 16, "graph_num_layers": 1, "max_nodes_in_batch": 120, "patience": PATIENCE, "random_seed": SEED})
 
 
 def scripted(task, fold, epoch, step, num_graphs, task_ids):
@@ -63,6 +67,30 @@ def write_qm9_folds(d):
             for r in part:
                 f.write(json.dumps(r) + "\n")
     return recs[:150], recs[150:]
+
+
+def write_qm9_data(d):
+    train_recs, valid_recs = write_qm9_folds(d)
+    test_file = os.path.join(d, "heldout.jsonl.gz")
+    with gzip.open(test_file, "wt") as f:
+        for r in (train_recs + valid_recs)[40:120]:
+            f.write(json.dumps(r) + "\n")
+    return train_recs, valid_recs, test_file
+
+
+def write_ppi_data(d):
+    BC.write_ppi_dir(d, "train", seed=1, num_graphs=9)
+    BC.write_ppi_dir(d, "valid", seed=2, num_graphs=4)
+    BC.write_ppi_dir(d, "test", seed=3, num_graphs=3)
+
+
+def recorded_reference_loop(key, d):
+    """The reference loop's log lines, feeds and best-model file as recorded with its data directory at ``{TMP}``."""
+    with open(RECORD) as f:
+        r = json.load(f)[key]
+    lines = [ln.replace("{TMP}", d) for ln in r["lines"]]
+    calls = [dict(c, first_feature_row=np.asarray(c["first_feature_row"], np.float32)) for c in r["calls"]]
+    return lines, calls, r["best_file"].replace("{TMP}", d), r["saved"]
 
 
 def run_reference_loop(task_name, data_dir, task_params, model_params, max_nodes=MAX_NODES, test_path=None):
@@ -191,16 +219,9 @@ def compare(ref_lines, ref_calls, pkg_lines, pkg_calls):
 
 
 def test_qm9_epoch_loop_writes_the_references_log(tmp_path):
-    train_recs, valid_recs = write_qm9_folds(str(tmp_path))
-    task_ids = [0, 4]
-    test_file = os.path.join(str(tmp_path), "heldout.jsonl.gz")
-    with gzip.open(test_file, "wt") as f:
-        for r in (train_recs + valid_recs)[40:120]:
-            f.write(json.dumps(r) + "\n")
-    ref_lines, ref_calls, best_file, saved = run_reference_loop(
-        "qm9", str(tmp_path), {"task_ids": task_ids},
-        {"hidden_size": 16, "graph_num_layers": 1, "max_nodes_in_batch": MAX_NODES, "patience": PATIENCE, "random_seed": SEED},
-        test_path=test_file)
+    train_recs, valid_recs, test_file = write_qm9_data(str(tmp_path))
+    task_ids = QM9_LOOP["task_params"]["task_ids"]
+    ref_lines, ref_calls, best_file, saved = recorded_reference_loop("qm9", str(tmp_path))
     assert saved
     L = batching.qm9_num_edge_types(train_recs + valid_recs)
     samples = lambda recs: [batching.qm9_graph_to_sample(r, L) for r in recs]
@@ -217,12 +238,8 @@ def test_qm9_epoch_loop_writes_the_references_log(tmp_path):
 
 def test_ppi_epoch_loop_writes_the_references_log(tmp_path):
     d = str(tmp_path)
-    BC.write_ppi_dir(d, "train", seed=1, num_graphs=9)
-    BC.write_ppi_dir(d, "valid", seed=2, num_graphs=4)
-    BC.write_ppi_dir(d, "test", seed=3, num_graphs=3)
-    ref_lines, ref_calls, best_file, saved = run_reference_loop(
-        "ppi", d, {}, {"hidden_size": 16, "graph_num_layers": 1, "max_nodes_in_batch": 120, "patience": PATIENCE, "random_seed": SEED},
-        max_nodes=120, test_path=d)
+    write_ppi_data(d)
+    ref_lines, ref_calls, best_file, saved = recorded_reference_loop("ppi", d)
     assert saved
     tr, _ = batching.load_ppi_fold(d, "train")
     va, _ = batching.load_ppi_fold(d, "valid")

@@ -45,15 +45,17 @@ def test_big_case_summary_bounds_follow_from_the_elementwise_tolerance():
     sys.path.insert(0, os.path.join(ROOT, "tests", "golden"))
     import ref_cases as RC
     rng = np.random.default_rng(0)
-    out = rng.standard_normal((1000, 64))
-    z = RC.summarize(out)
-    eps = 3e-5
-    noisy = out + eps * float(z["maxabs"]) * rng.uniform(-1, 1, size=out.shape)
-    assert max(RC.compare_with_summary(noisy, z)) <= eps
-    biased = out + eps * float(z["maxabs"])                                         # a systematic bias of eps is still within eps
-    assert max(RC.compare_with_summary(biased, z)) <= eps * (1 + 1e-9)
-    spoiled = out.copy(); spoiled[501, 7] += 1.0                                    # one bad element in an uncommitted row is seen
-    assert max(RC.compare_with_summary(spoiled, z)) > 1e-4
+    for shape in ((1000, 64), (30000, 8)):                                          # the second: thinned rows, block-summed projection
+        out = rng.standard_normal(shape)
+        z = RC.summarize(out)
+        assert ("proj_block" in z) == (shape[0] > RC.PROJ_BLOCK_ABOVE) and len(z["rows"]) <= RC.MAX_SUMMARY_ROWS
+        eps = 3e-5
+        noisy = out + eps * float(z["maxabs"]) * rng.uniform(-1, 1, size=out.shape)
+        assert max(RC.compare_with_summary(noisy, z)) <= eps
+        biased = out + eps * float(z["maxabs"])                                     # a systematic bias of eps is still within eps
+        assert max(RC.compare_with_summary(biased, z)) <= eps * (1 + 1e-9)
+        spoiled = out.copy(); spoiled[501, 7] += 1.0                                # one bad element in an uncommitted row is seen
+        assert max(RC.compare_with_summary(spoiled, z)) > 1e-4
 
 
 def test_tf1_optimizer_update_rules():

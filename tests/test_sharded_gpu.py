@@ -5,7 +5,7 @@
 * "virtual ranks" (SURVEY.md 4.4): all ranks of a partition live in this process on ONE GPU, each with its own stream; the
   pull exchange -- including its device-side cross-rank barrier and the epoch counter that makes it replayable -- runs for
   real, and a multi-layer sharded GNN-FiLM stack reproduces the numpy oracle on the whole graph at 1e-4.
-The same code on 2-8 real GPUs (CUDA-IPC peer memory over NVLink) is exercised by tools/sharded_check.py / bench.py --gpus N.
+The same code on 2-8 real GPUs (CUDA-IPC peer memory over NVLink) is exercised by bench.py --gpus N.
 """
 import numpy as np
 import pytest

@@ -31,7 +31,8 @@ from typing import Callable, Dict, List, Optional
 
 import numpy as np
 
-REFERENCE_ROOT = "/root/reference"
+# a checkout of the original microsoft/tf-gnn-samples: only the fixture generators under tests/golden execute it
+REFERENCE_ROOT = os.environ.get("TF_GNN_SAMPLES_REFERENCE", "")
 _F32_LOWEST = float(np.finfo(np.float32).min)
 
 
@@ -467,14 +468,16 @@ def installed(dtype=np.float64, seed: int = 0, provider: Optional[Callable] = No
         if k.split(".")[0] in _REFERENCE_MODULES:
             del sys.modules[k]
     sys.modules.update(mods)
-    sys.path.insert(0, reference_root)
+    if reference_root:
+        sys.path.insert(0, reference_root)
     import warnings
     try:
         with warnings.catch_warnings():
             warnings.simplefilter("ignore", SyntaxWarning)   # the reference's docstrings hold '\e' escapes (Python 3.12 warns)
             yield session
     finally:
-        sys.path.remove(reference_root)
+        if reference_root:
+            sys.path.remove(reference_root)
         for k in list(sys.modules):
             if k.split(".")[0] in _REFERENCE_MODULES or k in mods:
                 del sys.modules[k]

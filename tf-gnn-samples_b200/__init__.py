@@ -1,4 +1,4 @@
-"""b200-rgnn: B200-native relational GNN message passing behind the tf-gnn-samples layer API.
+"""b200-rgnn: H100-native relational GNN message passing behind the tf-gnn-samples layer API.
 
 Host code is Python over a C-ABI CUDA library (lib/librgnn.so, include/rgnn.h); torch tensors are
 the device-memory container.  There is NO CPU fallback: importing the layer functions works

@@ -40,13 +40,17 @@ void count_launch(int n = 1);
     if (_r != RGNN_OK) return _r;                                                          \
   } while (0)
 
+// SMs of an H100 SXM: the grid-shape heuristics (GEMM tile width, split-K, segment-kernel splits) aim at one wave of
+// this many CTAs; persistent grids use the SM count of the device they run on.
+constexpr int RGNN_WAVE_SMS = 132;
+
 static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 // ---- device-side activations: utils/utils.py:36-58 ----
 // The transcendental activations are kept OUT of line: inlining tanhf/erff/expm1f at every use site
-// (4 components x rows in flight x 2 sites) made the first segment kernel 26k SASS instructions and
-// instruction-fetch bound (profiles/r01_seg_reduce_v1.txt).  relu / linear / leaky_relu stay inline.
+// (4 components x rows in flight x 2 sites) makes the segment kernels many times larger and instruction-fetch
+// bound.  relu / linear / leaky_relu stay inline.
 // Each translation unit gets its own copy (static), so no relocatable device code is needed.
 // tanh is the default activation of GGNN / RGAT / the scaffold and sits in GEMM epilogues (GRU candidate state):
 // 1 - 2 / (exp(2x) + 1) with the SFU exponential -- absolute error < 1e-6 (the parity metric is max-norm, 1e-4),
@@ -93,8 +97,7 @@ __device__ __forceinline__ float4 act4(float4 v, int act) {
   if (act == RGNN_ACT_RELU) return make_float4(fmaxf(v.x, 0.0f), fmaxf(v.y, 0.0f), fmaxf(v.z, 0.0f), fmaxf(v.w, 0.0f));
   return slow_act4(v, act);
 }
-// Cold path (row epilogues, GEMM epilogue): nothing inline -- these kernels must stay under the ~2048-instruction
-// L1.5 I-cache (inlining tanh into the 8x-unrolled GEMM epilogue grew it to 2360 and cost 40 % on the FiLM config).
+// Cold path (row epilogues): nothing inline, to keep these kernels small enough for the instruction cache.
 __device__ __forceinline__ float4 act4_cold(float4 v, int act) {
   if (act == RGNN_ACT_LINEAR) return v;
   return slow_act4(v, act);
@@ -102,7 +105,7 @@ __device__ __forceinline__ float4 act4_cold(float4 v, int act) {
 
 // Programmatic dependent launch (sm_90+): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may
 // become resident while its predecessor in the stream is still running; pdl_wait() blocks until the predecessor grid has
-// COMPLETED and its writes are visible (no-op for a normal launch), so everything before it (barrier init, TMEM allocation,
+// COMPLETED and its writes are visible (no-op for a normal launch), so everything before it (barrier init,
 // reads of per-batch plan arrays) overlaps the predecessor's tail.  pdl_launch_dependents() lets the successor start.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

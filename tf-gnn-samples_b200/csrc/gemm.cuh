@@ -44,19 +44,19 @@ struct GemmParams {
   const int32_t* a_rows = nullptr;            // gathered A: output row r reads A1 row a_rows[r] (compact (source, type) transform)
 };
 
-// Blackwell path (gemm_tcgen05.cu): tcgen05.mma.kind::tf32 with a TMEM accumulator.  Needs scratch for
+// Hopper path (gemm_wgmma.cu): wgmma tf32 with register accumulators.  Needs scratch for
 // the pre-swizzled hi/lo weight images (gemm_tc_pack_bytes).  The scratch may be reused as soon as the call
 // returns as long as later users are ordered on the same stream.
 size_t gemm_tc_pack_bytes(const GemmParams& p);
 size_t gemm_tc_pack_bytes_uncached(const GemmParams& p);   // what a call needs when the weight-image cache is off
-int launch_gemm_tcgen05(const GemmParams& p, void* pack_ws, size_t pack_ws_bytes, cudaStream_t stream);
+int launch_gemm_tc(const GemmParams& p, void* pack_ws, size_t pack_ws_bytes, cudaStream_t stream);
 
 // Optional cache of the packed weight images (static weights).  See rgnn_set_weight_cache in include/rgnn.h.
 void gemm_weight_cache_enable(bool on);
 void gemm_weight_cache_clear();
 bool gemm_weight_cache_enabled();
 
-// C[M, N] = A^T . B, A [K, M] (lda), B [K, N] (ldb), K long (gemm_tn_tcgen05.cu): split-K over one wave of CTAs,
+// C[M, N] = A^T . B, A [K, M] (lda), B [K, N] (ldb), K long (gemm_tn_wgmma.cu): split-K over one wave of CTAs,
 // deterministic two-stage sum.  The result is written as N / block_cols column blocks, block b to ptr[b] (row
 // stride ld) -- one block per edge type for the per-type kernels' gradients.
 struct GemmTnOut {

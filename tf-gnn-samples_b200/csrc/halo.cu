@@ -483,7 +483,7 @@ static int halo_exchange_on(rgnn_halo_plan_t* hp, int buffer, int32_t d, cudaStr
   const long warps_needed = ((long)hp->n_halo + HALO_ROWS_IN_FLIGHT - 1) / HALO_ROWS_IN_FLIGHT;
   long ctas = (warps_needed + HALO_THREADS / 32 - 1) / (HALO_THREADS / 32);
   if (ctas < 1) ctas = 1;
-  if (ctas > 2 * 148) ctas = 2 * 148;
+  if (ctas > 2 * RGNN_WAVE_SMS) ctas = 2 * RGNN_WAVE_SMS;
   halo_pull_kernel<<<(unsigned)ctas, HALO_THREADS, 0, stream>>>(p);
   RGNN_CHECK_CUDA(cudaGetLastError());
   count_launch();

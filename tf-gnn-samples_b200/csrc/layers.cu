@@ -77,7 +77,7 @@ int check_ws(const Arena& a, const char* who) {
   return RGNN_OK;
 }
 
-// Dispatch one dense contraction on the tcgen05 kernel (weight images packed into arena scratch that is released
+// Dispatch one dense contraction on the wgmma kernel (weight images packed into arena scratch that is released
 // right after the enqueue -- later users are stream-ordered).
 int run_gemm(const GemmParams& g, Arena& ar, cudaStream_t stream) {
   const size_t need = gemm_tc_pack_bytes(g);
@@ -87,7 +87,7 @@ int run_gemm(const GemmParams& g, Arena& ar, cudaStream_t stream) {
     set_error("workspace too small for the weight images of a dense contraction (%zu bytes given, %zu needed)", ar.cap, ar.used);
     return RGNN_E_WORKSPACE;
   }
-  const int rc = launch_gemm_tcgen05(g, ws, need, stream);
+  const int rc = launch_gemm_tc(g, ws, need, stream);
   ar.used = mark;
   return rc;
 }
@@ -298,7 +298,7 @@ extern "C" size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, 
     case RGNN_LAYER_GGNN: floats = V * L * dm + 6 * V * dm; break;
     case RGNN_LAYER_RGAT: floats = V * L * dm + 2 * V * L * dm / 4 + 2 * V * dm; break;
     case RGNN_LAYER_FILM: floats = 3 * V * L * dm + 2 * V * dm; break;
-    case RGNN_LAYER_RGCN_BACKWARD: floats = 2 * V * L * dm + 2 * V * dm + (148 * 16384 + L * dm * dm) + 64 * 1024; break;   // + split-K partial tiles of dW
+    case RGNN_LAYER_RGCN_BACKWARD: floats = 2 * V * L * dm + 2 * V * dm + (RGNN_WAVE_SMS * 16384 + L * dm * dm) + 64 * 1024; break;   // + split-K partial tiles of dW
     case RGNN_LAYER_EDGE_MLP:
     case RGNN_LAYER_RGIN: {
       const size_t nl = (size_t)(mlp_layers > 0 ? mlp_layers : 1);
@@ -372,7 +372,7 @@ extern "C" int rgnn_rgcn_forward(const rgnn_plan_t* plan, const float* h, int32_
 // gnns/rgcn.py:84-114 (the reference trains through TF autodiff, models/sparse_graph_model.py:253-260).
 //   d_agg = grad_out * act'(.) / div            (elementwise)
 //   d_T[u, l, :] = sum_{(u->v) in A_l} s_{l,v} * d_agg[v, :]      (sorted-segment kernel over the reverse index)
-//   d_H = d_T . [W_0|...|W_{L-1}]^T             (tcgen05 GEMM, transposed weight images)
+//   d_H = d_T . [W_0|...|W_{L-1}]^T             (wgmma GEMM, transposed weight images)
 //   d_W_l = H^T . d_T[:, l, :]                  (tiled FMA kernel, deterministic two-stage sum)
 extern "C" int rgnn_rgcn_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d_in, int32_t d_out,
                                   const float* const* edge_weights, const float* num_incoming, int activation,
@@ -437,7 +437,7 @@ extern "C" int rgnn_rgcn_backward(const rgnn_plan_t* plan_c, const float* h, int
     RGNN_PROPAGATE(run_gemm(g, ar, stream));
   }
   if (grad_edge_weights != nullptr) {
-    // dW_l = H^T . dT[:, l, :]  -- one TN contraction over the V nodes for all types (gemm_tn_tcgen05.cu)
+    // dW_l = H^T . dT[:, l, :]  -- one TN contraction over the V nodes for all types (gemm_tn_wgmma.cu)
     GradWTable tab;
     GemmTnOut tn;
     tn.block_cols = d_out; tn.ld = d_out;
@@ -550,7 +550,7 @@ extern "C" int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* h, int32_
   float* T = ar.floats((size_t)V * L * D);
   float* m = ar.floats((size_t)V * D);
   static const int slab_env = getenv("RGNN_GRU_SLAB") ? atoi(getenv("RGNN_GRU_SLAB")) : 0;   // rows per slab (experiment knob)
-  const int slab_default = 148 * 128;                                         // one wave of 128-row tiles (measured: 18,944 rows 1.93 ms, 37,888 2.05, 56,832 2.23 on QM9-10k)
+  const int slab_default = RGNN_WAVE_SMS * 128;                               // one wave of 128-row tiles
   const int slab = slab_env > 0 ? slab_env : (V < slab_default ? (V > 0 ? V : 1) : slab_default);
   float* z = ar.floats((size_t)slab * D);
   float* rh = ar.floats((size_t)slab * D);
@@ -583,10 +583,9 @@ extern "C" int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* h, int32_
       RGNN_PROPAGATE(run_gemm(g, ar, stream));
     } else {                                                                  // GRUCell, gates z|r|h (A.4)
       // Two GEMMs per row SLAB: [z | r.h] = hs([m|h].[W_zr;U_zr] + b), then h' = z.h + (1-z).act([m | r.h].[W_h;U_h] + b_h).
-      // z and r.h live in slab-sized scratch that every slab overwrites: with ~19k rows per slab (one wave of 128-row
-      // tiles on 148 SMs) the slab's z, r.h, m, h and output rows (5 x 9.7 MB) stay in the 126 MB L2 between the two kernels and the
-      // dirty z / r.h lines are overwritten before they are evicted -- the round trip through HBM of round 1
-      // (4 x 92 MB per timestep on the QM9-10k batch) becomes L2 traffic.
+      // z and r.h live in slab-sized scratch that every slab overwrites: with ~17k rows per slab (one wave of 128-row
+      // tiles on 132 SMs) the slab's z, r.h, m, h and output rows (5 x 8.7 MB at D = 128) fit the 50 MB L2 between the two
+      // kernels, and the dirty z / r.h lines are overwritten before they are evicted instead of making a round trip through HBM.
       const int Vc = plan->Vt;
       for (int r0 = 0; r0 < Vc; r0 += slab) {
         const int rows = (Vc - r0 < slab) ? Vc - r0 : slab;

@@ -67,9 +67,8 @@ __device__ __forceinline__ void warp_layer_norm(float4 (&x)[NV], const bool (&ok
 // NV float4 per lane (the warp covers 128*NV columns starting at blockIdx.y * 128*NV); MODE = MsgMode;
 // MAXAGG = tf.unsorted_segment_max; SCALED = per-message 1/(c+1e-7); ACTMSG = activation applied per message.
 // Layer-norm epilogues need the whole row in one warp (gridDim.y == 1).
-// Code size matters here: the B200 SM has a ~32 KB (2048-instruction) L1.5 I-cache; variants of this kernel
-// above that size ran 1.5-2x slower at identical memory traffic (profiles/r01_seg_reduce_sweep.txt), so rare
-// paths are template flags (separate small kernels), not runtime branches, and nothing is duplicated.
+// Code size matters here: the SM's instruction cache is small, so rare paths are template flags (separate small
+// kernels), not runtime branches, and nothing is duplicated.
 template <int NV, int MODE, bool MAXAGG, bool SCALED, bool ACTMSG>
 __device__ __forceinline__ void seg_accumulate(const SegParams& p, int v, int col0, int lane, const bool (&ok)[NV],
                                                int beg, int end, int chunk0, int chunk_stride, float4 (&acc)[NV]) {
@@ -192,13 +191,11 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_kernel(const 
   seg_finish<NV>(p, v, col0, lane, ok, end - beg, acc);
 }
 
-// Small batches (V * D/128 warps do not fill the 148 SMs: the PPI-shaped single graph has 4,490) leave the warp-per-128-column
-// kernel latency-bound at ~40 % of the resident-warp limit (profiles/r01_final_kernels.txt).  Here a warp owns a 64-column
+// Small batches (V * D/128 warps do not fill the SMs: the PPI-shaped single graph has 4,490) can leave the warp-per-128-column
+// kernel latency-bound.  Here a warp owns a 64-column
 // slice and its two half-warps gather two DIFFERENT edges of the target per load instruction (each 16 lanes x 16 B = 256 B),
 // so the same bytes per instruction are in flight from twice as many warps; the two partial sums are combined with one
 // xor-16 shuffle round at the end (fixed order: deterministic).  Linear messages, sum / mean / sqrt_n only.
-// Measured (B200, PPI-shaped RGCN step, cold L2): 87.84 -> 87.55 us per 3-layer step, single cold layer 34.8 -> 33.5 us --
-// i.e. occupancy was NOT the limiter; the edge stage is bound by L2 -> SM delivery (DESIGN.md 5.3).  Kept (it is never slower).
 template <bool SCALED>
 __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_half_kernel(const __grid_constant__ SegParams p) {
   const int lane = threadIdx.x & 31, half = lane >> 4, l16 = lane & 15;
@@ -903,7 +900,7 @@ __global__ void grad_weight_reduce_kernel(const float* __restrict__ partial, int
 
 inline int grad_weight_splits(int V, int L, int d_in, int d_out) {
   const int tiles = ((d_in + GW_TILE - 1) / GW_TILE) * ((d_out + GW_TILE - 1) / GW_TILE) * L;
-  int splits = (2 * 148 + tiles - 1) / tiles;
+  int splits = (2 * RGNN_WAVE_SMS + tiles - 1) / tiles;
   const int max_by_rows = (V + 63) / 64;
   if (splits > max_by_rows) splits = max_by_rows;
   if (splits > 64) splits = 64;
@@ -934,12 +931,12 @@ static void launch_seg_pair(const SegParams& p, dim3 grid, cudaStream_t stream) 
     if (p.heavy_known > 0 && p.heavy_scratch != nullptr && p.heavy_items != nullptr) {
       const unsigned ix = p.heavy_items_known > 0 ? (unsigned)(p.heavy_items_known < 1184 ? p.heavy_items_known : 1184) : 296u;
       seg_reduce_heavy_part_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG><<<dim3(ix, grid.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-      const unsigned fx = p.heavy_known > 0 ? (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK) : 148u;
+      const unsigned fx = p.heavy_known > 0 ? (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK) : (unsigned)RGNN_WAVE_SMS;
       seg_reduce_heavy_finish_kernel<NV, MAXAGG><<<dim3(fx, grid.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
       count_launch(2);
       return;
     }
-    const unsigned gx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 592 ? p.heavy_known : 592) : 148u;
+    const unsigned gx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
     seg_reduce_heavy_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG><<<dim3(gx, grid.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
     count_launch();
   }
@@ -985,7 +982,7 @@ int launch_seg_reduce(const SegParams& p, cudaStream_t stream) {
     // warps, 73 us).  Reduce with one warp per 128-column slice instead and normalise the finished rows in a second, tiny
     // pass (V x D x 8 bytes; the layer-norm kernel works in place: it holds the row in registers).
     static const int ln_split_env = getenv("RGNN_LN_SPLIT") ? atoi(getenv("RGNN_LN_SPLIT")) : -1;   // 0 / 1 force
-    const bool ln_split = p.D > 128 && p.ld_out == p.D && (ln_split_env == 1 || (ln_split_env != 0 && (long)p.V < 148L * 40));
+    const bool ln_split = p.D > 128 && p.ld_out == p.D && (ln_split_env == 1 || (ln_split_env != 0 && (long)p.V < (long)RGNN_WAVE_SMS * 40));
     if (ln_split) {
       SegParams q = p;
       q.ln_gamma = nullptr; q.ln_beta = nullptr;
@@ -1008,7 +1005,7 @@ int launch_seg_reduce(const SegParams& p, cudaStream_t stream) {
     static const int half_env = getenv("RGNN_SEG_HALF") ? atoi(getenv("RGNN_SEG_HALF")) : -1;   // 0 / 1 force, default auto
     const long warps128 = (long)p.V * ((p.D + 127) / 128);
     const bool half_ok = p.msg_mode == MSG_LINEAR && p.agg != RGNN_AGG_MAX && p.act_msg == RGNN_ACT_LINEAR && p.D >= 64;
-    const bool use_half = half_ok && (half_env == 1 || (half_env != 0 && warps128 < 148L * 40));
+    const bool use_half = half_ok && (half_env == 1 || (half_env != 0 && warps128 < (long)RGNN_WAVE_SMS * 40));
     static const bool bulk_env = getenv("RGNN_SEG_BULK") != nullptr && atoi(getenv("RGNN_SEG_BULK")) == 1;   // experiment: TMA row gather
     if (bulk_env && half_ok && (p.stride_idx % 4) == 0) {
       const dim3 grid(gx, (p.D + 127) / 128);
@@ -1016,7 +1013,7 @@ int launch_seg_reduce(const SegParams& p, cudaStream_t stream) {
       else RGNN_CHECK_CUDA(launch_pdl(seg_reduce_bulk_kernel<false>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));
       count_launch();
       if (p.heavy_threshold > 0 && p.heavy_known != 0) {
-        const unsigned hx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 592 ? p.heavy_known : 592) : 148u;
+        const unsigned hx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
         const dim3 hgrid(hx, (p.D + 127) / 128);
         if (p.num_incoming != nullptr) seg_reduce_heavy_kernel<1, MSG_LINEAR, false, true, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
         else seg_reduce_heavy_kernel<1, MSG_LINEAR, false, false, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
@@ -1030,13 +1027,13 @@ int launch_seg_reduce(const SegParams& p, cudaStream_t stream) {
       if (p.heavy_threshold > 0 && p.heavy_known > 0 && p.heavy_scratch != nullptr && p.heavy_items != nullptr) {
         const dim3 g128(1, (p.D + 127) / 128);
         const unsigned ix = p.heavy_items_known > 0 ? (unsigned)(p.heavy_items_known < 1184 ? p.heavy_items_known : 1184) : 296u;
-        const unsigned fx = p.heavy_known > 0 ? (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK) : 148u;
+        const unsigned fx = p.heavy_known > 0 ? (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK) : (unsigned)RGNN_WAVE_SMS;
         if (p.num_incoming != nullptr) seg_reduce_heavy_part_kernel<1, MSG_LINEAR, false, true, false><<<dim3(ix, g128.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
         else seg_reduce_heavy_part_kernel<1, MSG_LINEAR, false, false, false><<<dim3(ix, g128.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
         seg_reduce_heavy_finish_kernel<1, false><<<dim3(fx, g128.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
         count_launch(2);
       } else if (p.heavy_threshold > 0 && p.heavy_known != 0) {   // heavy targets without scratch: one CTA per target
-        const unsigned hx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 592 ? p.heavy_known : 592) : 148u;
+        const unsigned hx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
         const dim3 hgrid(hx, (p.D + 127) / 128);
         if (p.num_incoming != nullptr) seg_reduce_heavy_kernel<1, MSG_LINEAR, false, true, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
         else seg_reduce_heavy_kernel<1, MSG_LINEAR, false, false, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
@@ -1061,7 +1058,7 @@ int launch_seg_rgat(const RgatParams& p, cudaStream_t stream) {
   const int lph = (p.D / p.K) / 4;
   static const int rgat_half_env = getenv("RGNN_RGAT_HALF") ? atoi(getenv("RGNN_RGAT_HALF")) : -1;   // 0 / 1 force, default: small batches
   const bool half_ok = p.s_src == nullptr && lph <= 16;
-  if (half_ok && (rgat_half_env == 1 || (rgat_half_env != 0 && (long)p.V * ((p.D + 127) / 128) < 148L * 40))) {
+  if (half_ok && (rgat_half_env == 1 || (rgat_half_env != 0 && (long)p.V * ((p.D + 127) / 128) < (long)RGNN_WAVE_SMS * 40))) {
     const dim3 hgrid(grid.x, (p.D + 63) / 64);
     RGNN_CHECK_CUDA(launch_pdl(seg_rgat_half_kernel, hgrid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));
   } else if (p.s_src == nullptr) RGNN_CHECK_CUDA(launch_pdl(seg_rgat_kernel<1, true>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));

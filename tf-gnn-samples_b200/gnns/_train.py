@@ -4,7 +4,7 @@ The inference paths of gnns/*.py are single fused library calls.  Under autograd
 sparse_rgcn_layer keeps its fused forward/backward kernels (rgnn_rgcn_backward); the other layers are composed here
 from the engine's differentiable building blocks (ops.py) --
 
-  * ops.dense            tcgen05 3xTF32 GEMM, both gradients on the tensor cores (transposed-weight GEMM, split-K TN);
+  * ops.dense            wgmma 3xTF32 GEMM, both gradients on the tensor cores (transposed-weight GEMM, split-K TN);
   * ops.edge_aggregate   the fused gather -> scale -> segment-reduce kernel on per-node tables [V, L, D] and its reverse
                          (segments = (source, type)) -- no per-edge tensor in either direction;
   * ops.segment_aggregate / ops.gather_rows / ops.gather_table_rows   for the layers whose messages are non-linear per

@@ -31,7 +31,7 @@ def _dense_raw(x, kernel, b, act_code):
 def dense_backward(x: torch.Tensor, kernel: torch.Tensor, grad_out: torch.Tensor, need_x: bool = True,
                    need_kernel: bool = True):
     """Gradients of y = x @ kernel: (grad_out @ kernel^T, x^T @ grad_out) through rgnn_dense_backward
-    (tcgen05 3xTF32; the x^T contraction is split-K over the rows, deterministic)."""
+    (wgmma 3xTF32; the x^T contraction is split-K over the rows, deterministic)."""
     x, kernel, g = as_f32(x, "x"), as_f32(kernel, "kernel"), as_f32(grad_out, "grad_out")
     gx = torch.empty_like(x) if need_x else None
     gk = torch.empty_like(kernel) if need_kernel else None
@@ -63,7 +63,7 @@ class _Linear(torch.autograd.Function):
 def dense(x: torch.Tensor, kernel: torch.Tensor, bias: Optional[torch.Tensor] = None,
           activation: Optional[str] = None) -> torch.Tensor:
     """act(x @ kernel + bias): tf.keras.layers.Dense with the Keras [in, out] kernel (SURVEY.md A.1),
-    fp32-accurate on the tensor cores (tcgen05 3xTF32).  Under autograd the contraction and both of its
+    fp32-accurate on the tensor cores (wgmma 3xTF32).  Under autograd the contraction and both of its
     gradients run on the engine (bias / activation are then applied by torch so that autograd can chain them)."""
     x, kernel = as_f32(x, "x"), as_f32(kernel, "kernel")
     if x.dim() != 2 or kernel.dim() != 2 or x.shape[1] != kernel.shape[0]:

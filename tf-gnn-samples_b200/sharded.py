@@ -191,7 +191,7 @@ class ShardedGraph:
         protocol, SURVEY.md 4.4): plain torch allocations, every rank sees every other rank's pointers directly.  The
         exchanges of the virtual ranks must then be enqueued on DIFFERENT streams (they wait for each other on the device),
         and all of their pull kernels must fit on the GPU at once (a rank's CTAs spin until every other rank's CTA 0 has run:
-        small test graphs only -- at most 296 CTAs of 512 threads per rank, 592 fit on a B200)."""
+        small test graphs only -- at most 264 CTAs of 512 threads per rank, 528 fit on an H100)."""
         lib = load_library()
         d = int(state_dim)
         world = len(graphs)
