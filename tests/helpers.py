@@ -48,6 +48,32 @@ def to_cuda_inputs(h, adj, indeg, device):
             None if indeg is None else torch.as_tensor(indeg).to(device))
 
 
+def launched_kernels(fn, expect=()):
+    """Run `fn` under torch.profiler with CUDA activities and return the set of demangled names of the kernels it launched
+    (CUPTI records every kernel of the process, including those launched by librgnn.so through ctypes).  A test asserts
+    the variant it means to exercise is among them, so a heuristic that later routes the shape elsewhere fails loudly.
+
+    The device trace has been seen to come back without some of the kernels a run launched (once without any).  The
+    window is padded on both sides, and while a name containing one of the `expect` substrings is missing `fn` is
+    profiled again, at most three times in all, so `fn` must be safe to repeat.  A kernel that is never launched is
+    still missing from the result."""
+    import time
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    names = set()
+    for _ in range(3):
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            time.sleep(0.05)
+            fn()
+            torch.cuda.synchronize()
+            time.sleep(0.05)
+        names |= {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA}
+        if names and all(any(s in n for n in names) for s in expect):
+            break
+    return names
+
+
 def assert_parity_8c(got, want64, want32, what=""):
     """SURVEY.md 8(c) acceptance, both clauses spelled out: max-norm relative error vs the float64 truth <= 1e-4 (north
     star) AND no worse than 10x the error the reference-order float32 arithmetic (`want32`) makes itself.  Deep stacks
