@@ -74,6 +74,73 @@ def launched_kernels(fn, expect=()):
     return names
 
 
+def rel(got, want):
+    """max |got - want| / max |want| (the absolute difference when want is all zeros)."""
+    want = np.asarray(want, np.float64)
+    scale = np.abs(want).max()
+    d = np.abs(np.asarray(got, np.float64) - want).max()
+    return float(d / scale) if scale > 0 else float(d)
+
+
+def to_dev(weights, device):
+    """numpy weight container -> the same container of float32 leaf tensors on `device` that require a gradient."""
+    import torch
+    if isinstance(weights, dict):
+        return {k: to_dev(v, device) for k, v in weights.items()}
+    if isinstance(weights, (list, tuple)):
+        return [to_dev(v, device) for v in weights]
+    if weights is None:
+        return None
+    return torch.as_tensor(np.ascontiguousarray(weights), dtype=torch.float32).to(device).requires_grad_(True)
+
+
+def compare(engine_fn, oracle_fn, h, w, proj_seed=0, tol=TOL, expect=None):
+    """engine_fn(h_dev, w_dev) / oracle_fn(h64, w64) -> output; compares output and d<out, proj>/d{h, every weight} with
+    torch float64 autograd over the reference op order (oracle/ref_autograd.py).  Returns ({name: error}, kernel names).
+
+    With `expect` (kernel-name substrings, see launched_kernels) only the backward pass is profiled -- the forward runs
+    outside the profiler, so every name returned was launched by a gradient -- and the kernel names are returned; without
+    it the name set is empty."""
+    import torch
+    from oracle import ref_autograd as A
+    dev = torch.device("cuda", 0)
+    hd = torch.as_tensor(h).to(dev).requires_grad_(True)
+    wd = to_dev(w, dev)
+    out = engine_fn(hd, wd)
+    proj = np.random.default_rng(proj_seed).standard_normal(tuple(out.shape)).astype(np.float32)
+    loss = (out * torch.as_tensor(proj).to(dev)).sum()
+    names = set()
+    if expect is None:
+        loss.backward()
+    else:
+        leaves = [hd] + list(A.flatten(wd).values())
+
+        def backward():                       # launched_kernels may run it up to three times: start each from no gradient
+            for t in leaves:
+                t.grad = None
+            loss.backward(retain_graph=True)
+        names = launched_kernels(backward, expect)
+    h64 = torch.as_tensor(h, dtype=torch.float64).requires_grad_(True)
+    w64 = A.to_torch64(w)
+    out64 = oracle_fn(h64, w64)
+    (out64 * torch.as_tensor(proj, dtype=torch.float64)).sum().backward()
+    errs = {"out": rel(out.detach().cpu().numpy(), out64.detach().numpy()), "d_h": rel(hd.grad.cpu().numpy(), h64.grad.numpy())}
+    fd, f64 = A.flatten(wd), A.flatten(w64)
+    assert list(fd) == list(f64)
+    for k in fd:
+        if f64[k].grad is None:
+            assert fd[k].grad is None or float(fd[k].grad.abs().max()) == 0.0, k
+            continue
+        if fd[k].grad is None:                                   # e.g. the kernel of an edge type without edges: autograd never sees it
+            assert float(f64[k].grad.abs().max()) == 0.0, "no gradient reached %s" % k
+            continue
+        errs["d_" + k] = rel(fd[k].grad.cpu().numpy(), f64[k].grad.numpy())
+    print({k: "%.1e" % v for k, v in errs.items()})
+    bad = {k: v for k, v in errs.items() if not v <= tol}
+    assert not bad, bad
+    return errs, names
+
+
 def assert_parity_8c(got, want64, want32, what=""):
     """SURVEY.md 8(c) acceptance, both clauses spelled out: max-norm relative error vs the float64 truth <= 1e-4 (north
     star) AND no worse than 10x the error the reference-order float32 arithmetic (`want32`) makes itself.  Deep stacks

@@ -9,59 +9,9 @@ from oracle import ref_autograd as A
 from tf_gnn_samples_b200 import (GraphPlan, batching, ops, sparse_ggnn_layer, sparse_gnn_edge_mlp_layer, sparse_gnn_film_layer,
                                  sparse_rgat_layer, sparse_rgcn_layer, sparse_rgin_layer, weights as W)
 
-from helpers import node_states, tiny_graph
+from helpers import compare, node_states, rel, tiny_graph, to_dev
 
 pytestmark = pytest.mark.gpu
-TOL = 1e-4
-
-
-def to_dev(weights, device):
-    import torch
-    if isinstance(weights, dict):
-        return {k: to_dev(v, device) for k, v in weights.items()}
-    if isinstance(weights, (list, tuple)):
-        return [to_dev(v, device) for v in weights]
-    if weights is None:
-        return None
-    return torch.as_tensor(np.ascontiguousarray(weights), dtype=torch.float32).to(device).requires_grad_(True)
-
-
-def compare(engine_fn, oracle_fn, h, w, proj_seed=0, tol=TOL):
-    """engine_fn(h_dev, w_dev) / oracle_fn(h64, w64) -> output; compares output and d<out, proj>/d{h, every weight}."""
-    import torch
-    dev = torch.device("cuda", 0)
-    hd = torch.as_tensor(h).to(dev).requires_grad_(True)
-    wd = to_dev(w, dev)
-    out = engine_fn(hd, wd)
-    proj = np.random.default_rng(proj_seed).standard_normal(tuple(out.shape)).astype(np.float32)
-    (out * torch.as_tensor(proj).to(dev)).sum().backward()
-    h64 = torch.as_tensor(h, dtype=torch.float64).requires_grad_(True)
-    w64 = A.to_torch64(w)
-    out64 = oracle_fn(h64, w64)
-    (out64 * torch.as_tensor(proj, dtype=torch.float64)).sum().backward()
-    errs = {"out": rel(out.detach().cpu().numpy(), out64.detach().numpy()), "d_h": rel(hd.grad.cpu().numpy(), h64.grad.numpy())}
-    fd, f64 = A.flatten(wd), A.flatten(w64)
-    assert list(fd) == list(f64)
-    for k in fd:
-        if f64[k].grad is None:
-            assert fd[k].grad is None or float(fd[k].grad.abs().max()) == 0.0, k
-            continue
-        if fd[k].grad is None:                                   # e.g. the kernel of an edge type without edges: autograd never sees it
-            assert float(f64[k].grad.abs().max()) == 0.0, "no gradient reached %s" % k
-            continue
-        errs["d_" + k] = rel(fd[k].grad.cpu().numpy(), f64[k].grad.numpy())
-    print({k: "%.1e" % v for k, v in errs.items()})
-    bad = {k: v for k, v in errs.items() if not v <= tol}
-    assert not bad, bad
-    return errs
-
-
-def rel(got, want):
-    want = np.asarray(want, np.float64)
-    scale = np.abs(want).max()
-    d = np.abs(np.asarray(got, np.float64) - want).max()
-    return float(d / scale) if scale > 0 else float(d)
-
 
 V, L, D = 61, 4, 32
 
@@ -79,8 +29,13 @@ def test_building_blocks(cuda_device):
     table = rng.standard_normal((V, L, D)).astype(np.float32)
     M = plan.num_edges
     data = rng.standard_normal((M, D)).astype(np.float32)
-    data[5] = data[4]                                        # a tie for the max gradient (rows 4, 5 share a target? not necessarily)
     src = np.concatenate([a[:, 0] for a in adj]).astype(np.int64); tgt = np.concatenate([a[:, 1] for a in adj]).astype(np.int64)
+    # a tie for the max gradient: a copy of row i inside its own segment, the maximum of that segment in some columns
+    i = 4
+    j = int(np.flatnonzero(tgt == tgt[i])[-1])
+    assert j != i and tgt[j] == tgt[i]
+    data[j] = data[i]
+    assert (data[i] == data[tgt == tgt[i]].max(axis=0)).any(), "row %d is the segment maximum in no column" % i
     typ = np.concatenate([np.full(a.shape[0], l, dtype=np.int64) for l, a in enumerate(adj)])
     cnt64 = torch.as_tensor(indeg, dtype=torch.float64)
     for agg in ["sum", "mean", "sqrt_n", "max"]:
