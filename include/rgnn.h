@@ -98,9 +98,10 @@ RGNN_API int rgnn_plan_create_ex(rgnn_plan_t** out, int32_t num_nodes, int32_t n
 RGNN_API int rgnn_plan_status(const rgnn_plan_t* plan);
 /* Sharded execution (one rank of a node-range partition: owned nodes first, halo nodes after them): declare that only
  * rows [0, num_targets) are targets whose outputs are wanted.  The edge stage then reduces only those rows and the
- * TARGET-side node-level work of the layers (FiLM's gamma/beta GEMM, GGNN's cell) runs on them only; source-side transforms
- * still cover all V rows.  Output rows >= num_targets are left untouched; layers must be called with num_timesteps == 1
- * (halo states are refreshed by the caller's exchange between steps).  Default: num_targets = V. */
+ * TARGET-side node-level work of the layers (FiLM's gamma/beta GEMM, GGNN's cell, RGDCN's dynamic kernels, RGIN's
+ * aggregation MLP and layer norm) runs on them only; source-side transforms still cover all V rows.  Output rows
+ * >= num_targets are left untouched; layers must be called with num_timesteps == 1 and rgnn_rgcn_stack_forward with
+ * num_layers == 1 (halo states are refreshed by the caller's exchange between steps).  Default: num_targets = V. */
 RGNN_API int rgnn_plan_set_num_targets(rgnn_plan_t* plan, int32_t num_targets);
 RGNN_API int rgnn_plan_destroy(rgnn_plan_t* plan);
 RGNN_API int32_t rgnn_plan_num_nodes(const rgnn_plan_t* plan);

@@ -459,6 +459,9 @@ extern "C" int rgnn_rgcn_stack_forward(const rgnn_plan_t* plan, const float* h, 
                                        size_t workspace_bytes, void* stream_) {
   RGNN_REQUIRE(plan != nullptr && num_layers >= 1, "rgcn_stack: plan is NULL or num_layers < 1");
   RGNN_REQUIRE(edge_weights != nullptr, "rgcn_stack: edge_weights is NULL");
+  // layer 2 would gather halo source rows of the intermediate buffer, which no layer of this call writes
+  RGNN_REQUIRE(num_layers == 1 || plan->Vt == plan->V,
+               "rgcn_stack: a plan restricted to %d of %d target rows supports num_layers == 1 only (halo rows are not updated)", plan->Vt, plan->V);
   const size_t row_bytes = align_up((size_t)plan->V * d * sizeof(float), 256);
   RGNN_REQUIRE(workspace != nullptr && workspace_bytes > 2 * row_bytes, "rgcn_stack: workspace too small");
   char* base = static_cast<char*>(workspace);
@@ -491,12 +494,12 @@ extern "C" int rgnn_rgdcn_forward(const rgnn_plan_t* plan, const float* h, int32
   RGNN_REQUIRE(num_channels >= 1 && num_channels <= RGNN_MAX_EDGE_TYPES && (d % num_channels) == 0,
                "rgdcn: num_channels %d must divide the state dim %d (and be <= %d)", num_channels, d, RGNN_MAX_EDGE_TYPES);
   RGNN_REQUIRE(!normalize || num_incoming != nullptr, "rgdcn: normalize_by_num_incoming needs type_to_num_incoming_edges");
-  const int V = plan->V, L = plan->L, C = num_channels, K = d / num_channels;
+  const int V = plan->V, Vt = plan->Vt, L = plan->L, C = num_channels, K = d / num_channels;
   RGNN_REQUIRE(K >= 4 && (K & (K - 1)) == 0 && K <= 128, "rgdcn: channel_dim %d must be a power of two in [4, 128]", K);
   for (int i = 0; i < L * C; ++i)
     RGNN_REQUIRE(channel_weights[i] != nullptr && aligned16(channel_weights[i]), "rgdcn: channel weight %d is NULL / misaligned", i);
   Arena ar(workspace, workspace_bytes);
-  float* wdyn = ar.floats((size_t)V * L * d * K);
+  float* wdyn = ar.floats((size_t)Vt * L * d * K);   // the dynamic kernels depend on the target: wanted target rows only
   float* buf[2] = {nullptr, nullptr};
   if (num_timesteps > 1) { buf[0] = ar.floats((size_t)V * d); buf[1] = ar.floats((size_t)V * d); }
   RGNN_PROPAGATE(check_ws(ar, "rgdcn"));
@@ -506,7 +509,7 @@ extern "C" int rgnn_rgdcn_forward(const rgnn_plan_t* plan, const float* h, int32
     // W[v, l, c] = act(F_{l,c} . input_v) reshaped [K, K]  (:139-148; the Dense carries the layer's activation, :101-103)
     for (int l = 0; l < L; ++l) {
       GemmParams g;
-      g.A1 = cur; g.lda1 = d; g.M = V; g.N = K * K; g.ldb1 = K * K;
+      g.A1 = cur; g.lda1 = d; g.M = Vt; g.N = K * K; g.ldb1 = K * K;
       g.C = wdyn + (size_t)l * d * K; g.ldc = L * d * K;
       g.act = activation; g.batch = C;
       for (int c = 0; c < C; ++c) { g.bptr[c] = channel_weights[l * C + c]; g.bptr2[c] = nullptr; }
@@ -515,9 +518,9 @@ extern "C" int rgnn_rgdcn_forward(const rgnn_plan_t* plan, const float* h, int32
       RGNN_PROPAGATE(run_gemm(g, ar, stream));
     }
     RgdcnParams r;
-    r.V = V; r.L = L; r.D = d; r.K = K;
+    r.V = Vt; r.L = L; r.D = d; r.K = K;
     r.seg_off = plan->seg_off; r.e_src = plan->e_src; r.e_type = plan->e_type;
-    r.h = cur; r.wdyn = wdyn; r.num_incoming = normalize ? num_incoming : nullptr;
+    r.h = cur; r.wdyn = wdyn; r.num_incoming = normalize ? num_incoming : nullptr; r.scale_ld = V;
     r.agg = aggregation; r.act_out = activation; r.out = dst;
     RGNN_PROPAGATE(launch_rgdcn_edges(r, stream));
     cur = dst;
@@ -655,7 +658,7 @@ extern "C" int rgnn_rgat_forward(const rgnn_plan_t* plan, const float* h, int32_
     RGNN_PROPAGATE(gemm_shared_a(ar, cur, V, din, edge_weights, L, D, D, T, RGNN_ACT_LINEAR, stream));   // rgat.py:95-96
     if (!fused_scores) RGNN_PROPAGATE(launch_rgat_scores(T, V, L, D, K, at, ssrc, stgt, stream));   // rgat.py:106-115 (per node)
     RgatParams r;
-    r.V = V; r.L = L; r.D = D; r.K = K; r.att = at;
+    r.V = plan->Vt; r.L = L; r.D = D; r.K = K; r.att = at;                  // T covers every source row, the softmax only the wanted targets
     r.seg_off = plan->seg_off; r.e_src = plan->e_src; r.e_type = plan->e_type;
     r.table = T; r.s_src = ssrc; r.s_tgt = stgt; r.act_out = activation; r.out = dst;
     RGNN_PROPAGATE(launch_seg_rgat(r, stream));                                                      // rgat.py:120-138
@@ -840,12 +843,12 @@ extern "C" int rgnn_rgin_forward(const rgnn_plan_t* plan, const float* h, int32_
         GemmParams g;
         g.A1 = prev; g.lda1 = aggr_dims[j]; g.K1 = aggr_dims[j];
         g.B1 = aggr_kernels[j]; g.ldb1 = aggr_dims[j + 1];
-        g.M = V; g.N = aggr_dims[j + 1]; g.C = next; g.ldc = aggr_dims[j + 1];
+        g.M = plan->Vt; g.N = aggr_dims[j + 1]; g.C = next; g.ldc = aggr_dims[j + 1];   // agg holds the wanted target rows only
         g.act = activation;   // hidden layers: MLP activation (rgin.py:80); last layer: the explicit activation of :138
         RGNN_PROPAGATE(run_gemm(g, ar, stream));
         prev = next;
       }
-      RGNN_PROPAGATE(launch_layer_norm(prev, V, D, ln_gamma + (size_t)t * D, ln_beta + (size_t)t * D, dst, stream));  // :139
+      RGNN_PROPAGATE(launch_layer_norm(prev, plan->Vt, D, ln_gamma + (size_t)t * D, ln_beta + (size_t)t * D, dst, stream));  // :139
     }
     cur = dst;
   }

@@ -71,7 +71,8 @@ struct RgdcnParams {
   const int32_t* e_type = nullptr;
   const float* h = nullptr;            // [V, D]
   const float* wdyn = nullptr;         // [V, L, D * K]
-  const float* num_incoming = nullptr; // [L, V] or NULL
+  const float* num_incoming = nullptr; // [L, scale_ld] or NULL
+  int scale_ld = 0;                    // row length of num_incoming (all graph nodes; V may be fewer wanted targets)
   int agg = RGNN_AGG_SUM;
   int act_out = RGNN_ACT_LINEAR;
   float* out = nullptr;                // [V, D]

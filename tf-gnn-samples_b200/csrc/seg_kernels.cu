@@ -344,6 +344,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_heavy_kernel(
   for (int k = 0; k < NV; ++k) ok[k] = (col0 + k * 128) < p.D;
   for (int i = blockIdx.x; i < nheavy; i += gridDim.x) {
     const int v = __ldg(p.heavy_list + i);
+    if (v >= p.V) continue;                             // not a wanted target (rgnn_plan_set_num_targets): row left untouched
     const int beg = __ldg(p.seg_off + v), end = __ldg(p.seg_off + v + 1);
     float4 acc[NV];
 #pragma unroll
@@ -382,6 +383,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_heavy_part_ke
   for (int it = blockIdx.x; it < nitems; it += gridDim.x) {
     const int2 vc = __ldg(reinterpret_cast<const int2*>(p.heavy_items) + it);
     const int v = vc.x;
+    if (v >= p.V) continue;                             // CTA-uniform: no __syncthreads is skipped by part of the block
     const int seg_end = __ldg(p.seg_off + v + 1);
     const int beg = __ldg(p.seg_off + v) + vc.y * p.heavy_chunk;
     const int end = min(seg_end, beg + p.heavy_chunk);
@@ -415,6 +417,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_heavy_finish_
   for (int k = 0; k < NV; ++k) ok[k] = (col0 + k * 128) < p.D;
   for (int i = blockIdx.x * WARPS_PER_BLOCK + (threadIdx.x >> 5); i < nheavy; i += gridDim.x * WARPS_PER_BLOCK) {
     const int v = __ldg(p.heavy_list + i);
+    if (v >= p.V) continue;
     const int deg = __ldg(p.seg_off + v + 1) - __ldg(p.seg_off + v);
     const int base = __ldg(p.heavy_base + i), n = (deg + p.heavy_chunk - 1) / p.heavy_chunk;
     float4 acc[NV];
@@ -483,7 +486,7 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) rgdcn_edge_kernel(const 
     run[k] = f4(0.0f);
   }
   int cur_type = -1;
-  auto scale_of = [&](int ty) { return p.num_incoming != nullptr ? 1.0f / (__ldg(p.num_incoming + (size_t)ty * p.V + v) + 1e-7f) : 1.0f; };
+  auto scale_of = [&](int ty) { return p.num_incoming != nullptr ? 1.0f / (__ldg(p.num_incoming + (size_t)ty * p.scale_ld + v) + 1e-7f) : 1.0f; };
   for (int e0 = beg; e0 < end; e0 += 32) {
     const int n = min(32, end - e0);
     int my_src = 0, my_type = 0;

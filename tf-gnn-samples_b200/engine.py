@@ -310,25 +310,35 @@ class GraphPlan:
             cache[key] = make()
         return cache[key]
 
+    def _lists(self) -> List[torch.Tensor]:
+        """The adjacency lists the plan was built from; a plan wrapped around a device-built handle has none."""
+        if self.adjacency_lists is None:
+            raise RgnnError(RGNN_E_INVALID,
+                            "this plan wraps a graph built inside the library (ShardedGraph.plan) and has no adjacency lists, "
+                            "which the differentiable (training) layer paths need.  To train on a node-range partition, use "
+                            "GraphPlan(NodeRangePartition.local_adjacency_lists, n_local).set_num_targets(n_own) with the "
+                            "states exchanged by NodeRangePartition.exchange")
+        return self.adjacency_lists
+
     @property
     def message_sources(self) -> torch.Tensor:
         """int64 [M]: source of every message, type-major concatenation order (gnns/rgcn.py:85,108)."""
-        return self._cached("src", lambda: torch.cat([a[:, 0] for a in self.adjacency_lists]).long())
+        return self._cached("src", lambda: torch.cat([a[:, 0] for a in self._lists()]).long())
 
     @property
     def message_targets(self) -> torch.Tensor:
         """int64 [M]: target of every message (gnns/rgcn.py:78)."""
-        return self._cached("tgt", lambda: torch.cat([a[:, 1] for a in self.adjacency_lists]).long())
+        return self._cached("tgt", lambda: torch.cat([a[:, 1] for a in self._lists()]).long())
 
     @property
     def message_types(self) -> torch.Tensor:
         return self._cached("typ", lambda: torch.cat([torch.full((a.shape[0],), l, dtype=torch.long, device=self.device)
-                                                      for l, a in enumerate(self.adjacency_lists)]))
+                                                      for l, a in enumerate(self._lists())]))
 
     @property
     def type_offsets(self) -> List[int]:
         off = [0]
-        for a in self.adjacency_lists:
+        for a in self._lists():
             off.append(off[-1] + int(a.shape[0]))
         return off
 
@@ -345,7 +355,7 @@ class GraphPlan:
 
         def make():
             lists = []
-            for l, a in enumerate(self.adjacency_lists):
+            for l, a in enumerate(self._lists()):
                 src, tgt = a[:, 0], a[:, 1]
                 if by == "source":
                     lists.append(torch.stack([tgt, src], dim=1))

@@ -98,7 +98,11 @@ def degree_balanced_cuts(adjacency_lists: Sequence[np.ndarray], num_nodes: int, 
 
 
 class ShardedGraph:
-    """Rank-local structure of a node-range partition, built on the device by rgnn_halo_plan_create."""
+    """Rank-local structure of a node-range partition, built on the device by rgnn_halo_plan_create.
+
+    ``plan`` carries no adjacency lists, so the layer paths that need them (the differentiable FiLM, RGAT, Edge-MLP,
+    RGIN and composed RGCN) refuse it with an RgnnError.  Training on a node-range partition uses a GraphPlan over
+    ``NodeRangePartition.local_adjacency_lists`` with ``set_num_targets(n_own)`` and ``NodeRangePartition.exchange``."""
 
     def __init__(self, adjacency_lists: Sequence, cuts: Sequence[int], rank: int, world: int,
                  device: Optional[torch.device] = None, group=None):
