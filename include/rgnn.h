@@ -17,9 +17,25 @@
  *             (pointer lists, sizes).  The library borrows pointers for the duration of the
  *             call only.  Plans own their index buffers.
  *   async     all work is enqueued on `stream` (a cudaStream_t passed as void*); forwards
- *             make no hidden synchronisation and are CUDA-Graph capturable.  plan_create
- *             synchronises the stream once (it sizes its buffers on the host).
- *   threads   re-entrant on distinct plans/streams; one plan must not be used concurrently.
+ *             make no hidden synchronisation and are CUDA-Graph capturable.  Calls that synchronise
+ *             (and return RGNN_E_INVALID, recording nothing, on a capturing stream): rgnn_plan_create /
+ *             _create_ex without RGNN_PLAN_DEFERRED_CHECK, rgnn_plan_status (on the creation stream).
+ *             rgnn_halo_plan_create also synchronises, and rgnn_weight_cache_clear /
+ *             rgnn_set_weight_cache(0) call cudaFree: never call them during a capture.
+ *   capture   run eagerly once before capturing: every layer with the weight cache on (a cache miss
+ *             during capture is an error), and the first backward on a plan (rgnn_rgcn_backward /
+ *             rgnn_edge_aggregate_backward build the plan's reverse index then; inside a capture they
+ *             return RGNN_E_INVALID).  A plan built with RGNN_PLAN_DEFERRED_CHECK inside a capture is
+ *             filled only when the graph is replayed: call rgnn_plan_status after a replay.  A graph
+ *             captured with the weight cache on reads the cached images: rgnn_weight_cache_clear (and
+ *             rgnn_set_weight_cache(0)) frees them, so such a graph must not be replayed afterwards.
+ *   threads   re-entrant on distinct plans/streams; one plan must not be used concurrently by two host
+ *             threads.  A plan may be used on streams other than its creation stream: order them after
+ *             the build (a deferred build is still running on the creation stream; a validated one has
+ *             finished).  rgnn_plan_destroy frees the plan stream-ordered on the CREATION stream: before
+ *             calling it, make that stream wait (event) for the work queued on every other stream that
+ *             uses the plan, or the memory may be handed to the next allocation (the next batch's plan)
+ *             while that work still reads it.  The Python GraphPlan does both itself.
  *   layouts   node states [V, D] fp32 row-major, D % 4 == 0; adjacency lists int32 [E_l, 2]
  *             (col 0 = source, col 1 = target: gnns/rgcn.py:85-86); in-degrees fp32 [L, V]
  *             (tasks/sparse_graph_task.py:145); weights in Keras orientation kernel[in, out]

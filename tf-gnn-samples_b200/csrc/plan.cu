@@ -155,6 +155,13 @@ int bits_for(uint64_t n) {   // number of low bits needed to represent values < 
 
 int plan_ensure_reverse(rgnn_plan* plan, cudaStream_t stream) {
   if (plan->rev_seg_off != nullptr) return RGNN_OK;
+  // Inside a capture the allocation below would be a graph allocation, unbacked and unfilled until the graph is replayed,
+  // yet kept by the plan for every later (eager) backward: refuse before anything is recorded.
+  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+  RGNN_CHECK_CUDA(cudaStreamIsCapturing(stream, &cap));
+  RGNN_REQUIRE(cap == cudaStreamCaptureStatusNone,
+               "backward: the first backward on a plan builds its reverse index, which cannot happen during CUDA-graph "
+               "capture (run one backward on this plan eagerly before capturing)");
   const int V = plan->V, L = plan->L;
   const int M = (int)plan->M;
   const size_t segments = (size_t)V * L;
@@ -236,6 +243,13 @@ extern "C" int rgnn_plan_create_ex(rgnn_plan_t** out, int32_t num_nodes, int32_t
                "plan_create: num_edge_types %d outside [1, %d]", num_edge_types, RGNN_MAX_EDGE_TYPES);
   RGNN_REQUIRE(adjacency_lists != nullptr && num_edges != nullptr, "plan_create: NULL adjacency table");
   RGNN_REQUIRE((uint64_t)num_nodes * (uint64_t)num_edge_types < (1ull << 32), "plan_create: V*L must be < 2^32");
+  if (!deferred) {   // the validated build synchronises the stream, which would invalidate a capture halfway through
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    RGNN_CHECK_CUDA(cudaStreamIsCapturing(stream, &cap));
+    RGNN_REQUIRE(cap == cudaStreamCaptureStatusNone,
+                 "plan_create: a validated build synchronises the stream and cannot be captured into a CUDA graph "
+                 "(build with RGNN_PLAN_DEFERRED_CHECK inside a capture)");
+  }
 
   AdjTable tab;
   int64_t M = 0;
@@ -414,6 +428,13 @@ extern "C" int rgnn_plan_create_ex(rgnn_plan_t** out, int32_t num_nodes, int32_t
 extern "C" int rgnn_plan_status(const rgnn_plan_t* plan) {
   RGNN_REQUIRE(plan != nullptr, "plan_status: plan is NULL");
   if (plan->err_flag == nullptr) return RGNN_OK;
+  {
+    cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
+    RGNN_CHECK_CUDA(cudaStreamIsCapturing(plan->stream, &cap));
+    RGNN_REQUIRE(cap == cudaStreamCaptureStatusNone,
+                 "plan_status: synchronises the plan's creation stream, which is capturing a CUDA graph (call it after "
+                 "the capture, once the graph has been replayed)");
+  }
   int flags[4] = {0, 0, 0, 0};
   RGNN_CHECK_CUDA(cudaMemcpyAsync(flags, plan->err_flag, 4 * sizeof(int), cudaMemcpyDeviceToHost, plan->stream));
   rgnn_plan* mp = const_cast<rgnn_plan*>(plan);
@@ -440,7 +461,9 @@ extern "C" int rgnn_plan_destroy(rgnn_plan_t* plan) {
   if (plan == nullptr) return RGNN_OK;
   if (plan->rev_block != nullptr) cudaFreeAsync(plan->rev_block, plan->stream);
   if (plan->pair_block != nullptr) cudaFreeAsync(plan->pair_block, plan->stream);
-  if (plan->block != nullptr) cudaFreeAsync(plan->block, plan->stream);   // stream-ordered: safe after queued forwards
+  // stream-ordered on the creation stream: safe after work queued on THAT stream; work on other streams must be ordered
+  // before this call by the caller (include/rgnn.h "threads")
+  if (plan->block != nullptr) cudaFreeAsync(plan->block, plan->stream);
   delete plan;
   return RGNN_OK;
 }

@@ -142,18 +142,29 @@ _weight_cache_on = False
 _weight_versions: Dict[int, tuple] = {}
 
 
+def refuse_under_capture(what: str):
+    """Raise RgnnError if the current stream is capturing a CUDA graph: for the calls that synchronise or free device
+    memory, which would otherwise invalidate the capture halfway through."""
+    if torch.cuda.is_available() and torch.cuda.is_current_stream_capturing():
+        raise RgnnError(RGNN_E_INVALID, "%s cannot run during CUDA-graph capture" % what)
+
+
 def set_weight_cache(enable: bool):
     """Static-weight mode (inference / benchmarking): keep the GEMM's packed weight images across calls
     (rgnn_set_weight_cache in include/rgnn.h).  The library keys the images on device POINTERS; this layer makes that
     safe: an in-place update (``Tensor._version`` changed) or the death of the tensor that owned a cached address
-    (its memory may since belong to a different weight) flushes the cache the next time that address is passed down."""
+    (its memory may since belong to a different weight) flushes the cache the next time that address is passed down.
+    Turning the cache off clears it, and clearing it frees the images that CUDA graphs captured with the cache on read:
+    such graphs must not be replayed afterwards."""
     global _weight_cache_on
+    refuse_under_capture("set_weight_cache (it clears the weight cache with cudaFree)")
     check(load_library().rgnn_set_weight_cache(1 if enable else 0))
     _weight_cache_on = bool(enable)
     _weight_versions.clear()
 
 
 def weight_cache_clear():
+    refuse_under_capture("weight_cache_clear (cudaFree)")
     check(load_library().rgnn_weight_cache_clear())
     _weight_versions.clear()
 
@@ -172,21 +183,24 @@ def note_weights(tensors):
     import weakref
     stale = False
     for t in tensors:
-        key, ver = t.data_ptr(), t._version
-        old = _weight_versions.get(key)
+        old = _weight_versions.get(t.data_ptr())
         if old is not None:
             old_ver, old_ref = old
             owner = old_ref()
             # a dead owner means the address may have been recycled for a different weight; a live but different owner at
             # the same address IS a different allocation (two live tensors cannot overlap unless they share a base)
-            if owner is None or old_ver != ver or owner is not _owner(t):
+            if owner is None or old_ver != t._version or owner is not _owner(t):
                 stale = True
-        _weight_versions[key] = (ver, weakref.ref(_owner(t)))
-    if len(_weight_versions) > 4096:                      # forget addresses whose owners are gone
-        for k in [k for k, (_, r) in _weight_versions.items() if r() is None]:
-            stale = True
-            del _weight_versions[k]
-    if stale:
+    dead = [k for k, (_, r) in _weight_versions.items() if r() is None] if len(_weight_versions) > 4096 else []
+    if stale or dead:
+        # checked before any bookkeeping changes, so that the next eager call still sees the weight as stale
+        refuse_under_capture("flushing the weight cache (a weight changed in place or was reallocated since it was "
+                             "cached; the flush calls cudaFree)")
+    for t in tensors:
+        _weight_versions[t.data_ptr()] = (t._version, weakref.ref(_owner(t)))
+    for k in dead:                                        # forget addresses whose owners are gone
+        del _weight_versions[k]
+    if stale or dead:
         check(load_library().rgnn_weight_cache_clear())
 
 
@@ -248,7 +262,14 @@ class GraphPlan:
     def __init__(self, adjacency_lists: Sequence, num_nodes: int, device: Optional[torch.device] = None,
                  validate: bool = True):
         """validate=True: synchronise and raise RgnnError if an adjacency list holds a node id outside [0, V)
-        (what TF does at sess.run).  validate=False: fully asynchronous build; ``check()`` reports later."""
+        (what TF does at sess.run).  validate=False: fully asynchronous build; ``check()`` reports later.
+
+        The plan is built on the current stream and may be used on any stream: the first use on another stream waits for
+        the build, and ``close()`` frees the plan after the work queued on every stream it was used on.  Inside a
+        CUDA-graph capture only validate=False is allowed (validation synchronises)."""
+        if validate:
+            refuse_under_capture("GraphPlan(validate=True) (it synchronises the stream; build with validate=False inside "
+                                 "a capture)")
         lib = load_library()
         adj: List[torch.Tensor] = []
         for a in adjacency_lists:
@@ -276,9 +297,17 @@ class GraphPlan:
         counts = (c_int64 * max(len(dev_adj), 1))(*[int(a.shape[0]) for a in dev_adj])
         ptrs = ptr_table(dev_adj, weights=False)
         handle = c_void_p()
+        self._stream = torch.cuda.current_stream(device)      # creation stream: the library frees the plan on it
+        self._other_streams: Dict[int, torch.cuda.Stream] = {}
+        self._built = None
         with torch.cuda.device(device):
             check(lib.rgnn_plan_create_ex(ctypes.byref(handle), self.num_nodes, self.num_edge_types, ptrs, counts,
-                                          0 if validate else 1, current_stream_ptr(device)))
+                                          0 if validate else 1, self._stream.cuda_stream))
+            if not validate and not torch.cuda.is_current_stream_capturing():
+                # a deferred build is still running on the creation stream: other streams wait for this event first (an
+                # event recorded during a capture cannot be waited on eagerly; a captured build is ordered by its graph)
+                self._built = torch.cuda.Event()
+                self._built.record(self._stream)
         self._handle = handle
         self.num_edges = int(lib.rgnn_plan_num_edges(handle))
 
@@ -301,12 +330,33 @@ class GraphPlan:
     def handle(self):
         if self._handle is None:
             raise RgnnError(RGNN_E_INVALID, "GraphPlan used after close()")
+        self._note_stream()
         return self._handle
+
+    def _note_stream(self):
+        """Called before work that reads the plan is queued on the current stream.  On a stream other than the creation
+        stream, the first use waits for a deferred build and the stream is remembered for close().  Work queued during a
+        CUDA-graph capture runs at replay, on the replaying stream: the caller keeps the plan alive while the graph is used."""
+        stream = getattr(self, "_stream", None)
+        if stream is None:                                     # a borrowed handle: its owner orders its lifetime
+            return
+        s = torch.cuda.current_stream(self.device)
+        if s.cuda_stream == stream.cuda_stream or s.cuda_stream in self._other_streams:
+            return
+        if torch.cuda.is_current_stream_capturing():
+            return
+        if self._built is not None:
+            s.wait_event(self._built)
+        self._other_streams[s.cuda_stream] = s
 
     # ---- index views used by the differentiable building blocks (ops.py); built lazily, cached ----
     def _cached(self, key, make):
         cache = self.__dict__.setdefault("_derived", {})
         if key not in cache:
+            # what make() records in a capture is computed only when the graph replays, but the cache would keep it for
+            # every later eager call (and torch.bincount synchronises): build the views eagerly, before capturing
+            refuse_under_capture("building the plan's index views / regrouped plans for the training paths on first use "
+                                 "(run one forward and backward on this plan eagerly before capturing)")
             cache[key] = make()
         return cache[key]
 
@@ -318,6 +368,7 @@ class GraphPlan:
                             "which the differentiable (training) layer paths need.  To train on a node-range partition, use "
                             "GraphPlan(NodeRangePartition.local_adjacency_lists, n_local).set_num_targets(n_own) with the "
                             "states exchanged by NodeRangePartition.exchange")
+        self._note_stream()
         return self.adjacency_lists
 
     @property
@@ -399,10 +450,24 @@ class GraphPlan:
         return out
 
     def close(self):
+        """Free the plan.  The library frees it stream-ordered on the creation stream; that stream first waits for the
+        work queued so far on every other stream the plan was used on (else the next allocation on the creation stream,
+        typically the next batch's plan, could reuse the memory while that work still reads it)."""
         if getattr(self, "_handle", None) is not None:
             if not getattr(self, "_borrowed", False):
-                load_library().rgnn_plan_destroy(self._handle)
+                if torch.cuda.is_current_stream_capturing():
+                    # e.g. the previous batch's plan garbage-collected inside a capture: freeing it now would invalidate
+                    # the capture, so it is freed by the next close() outside one
+                    _capture_pending.append(self._close_args())
+                else:
+                    for args in _capture_pending + [self._close_args()]:
+                        _destroy(*args)
+                    _capture_pending.clear()
             self._handle = None
+
+    def _close_args(self):
+        return self._handle, getattr(self, "_stream", None), list(getattr(self, "_other_streams", {}).values()), \
+            self.adjacency_lists or []
 
     def __del__(self):
         try:
@@ -417,10 +482,23 @@ class GraphPlan:
         self.close()
 
 
+_capture_pending: List[tuple] = []     # plans closed during a CUDA-graph capture, freed by the next close() outside one
+
+
+def _destroy(handle, stream, other_streams, adjacency_lists):
+    for s in other_streams:
+        stream.wait_stream(s)
+        for a in adjacency_lists:
+            a.record_stream(s)
+    load_library().rgnn_plan_destroy(handle)
+
+
 def resolve_plan(node_embeddings: torch.Tensor, adjacency_lists, plan: Optional[GraphPlan]) -> GraphPlan:
     """Layer functions accept either raw adjacency lists (reference call convention) or a GraphPlan."""
     if plan is not None:
         return plan
     if isinstance(adjacency_lists, GraphPlan):
         return adjacency_lists
+    refuse_under_capture("a layer called with raw adjacency lists (it builds and validates a plan, which synchronises; "
+                         "pass a GraphPlan built before the capture)")
     return GraphPlan(adjacency_lists, node_embeddings.shape[0], device=node_embeddings.device)
