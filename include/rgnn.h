@@ -282,6 +282,56 @@ RGNN_API int rgnn_halo_exchange(rgnn_halo_plan_t* plan, int buffer, int32_t d, v
  * that GEMM overlaps the transfer over NVLink.  Capturable into a CUDA graph (fork / join through events). */
 RGNN_API int rgnn_halo_exchange_overlapped(rgnn_halo_plan_t* plan, int buffer, int32_t d, void* stream);
 
+/* Training over the partition: the transpose of rgnn_halo_exchange.  A rank's layers produce gradients for its local rows
+ * [n_own + n_halo, d]; the rows >= n_own belong to other ranks and must be ADDED to their owners' rows.  The same
+ * peer-memory design carries them back, with no host-side index and no NCCL call on the data path.
+ *
+ * rgnn_halo_plan_attach_grad: like rgnn_halo_plan_attach, for the backward direction.  Every rank keeps TWO gradient
+ * buffers of [n_own + n_halo, d] floats (16-byte aligned; consecutive backward exchanges alternate them, as consecutive
+ * forward exchanges alternate the state buffers), a flag array uint32[world] that must start zeroed and must NOT be the
+ * forward exchange's (the two barriers never satisfy each other), and a halo list of int32 [4 + 2 * n_halo] (16-byte
+ * aligned).  The call writes this rank's halo list there ([0] = n_halo, [4, 4 + n_halo) = owners, [4 + n_halo,
+ * 4 + 2 n_halo) = rows in the owners' buffers) and synchronises.  All pointer arrays are host arrays of `world` device
+ * pointers valid in this process, entry [rank] = this rank's own memory.
+ *
+ * rgnn_halo_plan_build_reverse: once EVERY rank has returned from rgnn_halo_plan_attach_grad (a host-side barrier, e.g.
+ * torch.distributed.barrier), each rank reads its peers' published lists and builds on the device the reverse index:
+ * for every owned row, the (peer, row of that peer's gradient buffer) pairs that hold it as a halo row, sorted by (owned
+ * row, peer rank).  Synchronises `stream`; returns RGNN_E_INVALID, recording nothing, on a capturing stream.  Run it
+ * eagerly once per batch (per halo plan), before any capture.  rgnn_halo_plan_num_reverse: number of pairs (-1 before
+ * the build); rgnn_halo_plan_export_reverse copies the index into caller DEVICE buffers (any may be NULL): offsets
+ * [n_own + 1], peer and row [num_reverse].
+ *
+ * rgnn_halo_exchange_backward: grad_own[r] = grad_local[r] + the consumers' gradients of row r, added in ascending peer
+ * rank (a fixed order: bit-reproducible, no atomics); a row that no peer consumes is copied bit for bit.  grad_local
+ * [n_own + n_halo, d] is read (its halo rows are first copied into this rank's gradient buffer `buffer`, unless
+ * grad_local IS that buffer), grad_own [n_own, d] is written.  Collective, with rgnn_halo_exchange's discipline: every
+ * rank calls it the same number of times, in the same order, typically in the reverse order of the forward exchanges with
+ * the same buffer parity.  Capturable into a CUDA graph once the reverse index exists; its epoch lives on the device.  A
+ * peer that never arrives faults the kernel after 10 s.
+ *
+ * Calling order per batch: rgnn_halo_plan_create, rgnn_halo_plan_attach + rgnn_halo_plan_attach_grad, host barrier,
+ * rgnn_halo_plan_build_reverse; then per step: forward = { write owned rows into states(t % 2), rgnn_halo_exchange,
+ * layer t } for every layer, backward = { layer t backward on rgnn_halo_plan_graph's local graph,
+ * rgnn_halo_exchange_backward(t % 2) } from the last layer down.  Only the halo traffic is handled here: the weight
+ * gradients are still summed over the ranks by the caller (an all-reduce; scaffold.all_reduce_gradients_ in Python).
+ *
+ * Several ranks in one process on one GPU ("virtual ranks", tests): enqueue each rank's work on its own stream, make no
+ * call that waits for the device between a rank's exchanges, and keep every rank's exchange kernels co-resident (each
+ * launches at most ceil(rows / 128) CTAs of 512 threads, capped at 264 -- rows = n_halo forward, n_own backward; an H100
+ * holds 528 such CTAs in all): a rank's CTAs spin until every other rank's first CTA has run.  CUDA loads a kernel at its
+ * first launch (lazy module loading, the default) and that load can wait for the running kernels, a spinning exchange
+ * included: launch every other kernel of the step once before the ranks' exchanges, and enqueue the ranks phase by phase
+ * (every rank's exchange before any rank's next kernel).  rgnn_halo_plan_attach_grad loads the two exchange kernels. */
+RGNN_API int rgnn_halo_plan_attach_grad(rgnn_halo_plan_t* plan, void* const* peer_grads0, void* const* peer_grads1,
+                               void* const* peer_grad_flags, void* const* peer_halo_lists);
+RGNN_API int rgnn_halo_plan_build_reverse(rgnn_halo_plan_t* plan, void* stream);
+RGNN_API int64_t rgnn_halo_plan_num_reverse(const rgnn_halo_plan_t* plan);
+RGNN_API int rgnn_halo_plan_export_reverse(const rgnn_halo_plan_t* plan, int32_t* offsets, int32_t* peer, int32_t* row,
+                                  void* stream);
+RGNN_API int rgnn_halo_exchange_backward(rgnn_halo_plan_t* plan, int buffer, int32_t d, const float* grad_local,
+                                float* grad_own, void* stream);
+
 /* CUDA-IPC plumbing for the above (one node): allocate zeroed device memory that peers can map, export its 64-byte handle
  * (ship it with any host-side channel, e.g. torch.distributed.all_gather_object), map a peer's allocation. */
 RGNN_API int rgnn_peer_alloc(void** ptr, size_t bytes, void* handle_out /* RGNN_PEER_HANDLE_BYTES */);

@@ -79,6 +79,11 @@ SIGNATURES = {
     "rgnn_halo_plan_attach": (c_int, [_PTR, _PTR, _PTR, _PTR]),
     "rgnn_halo_exchange": (c_int, [_PTR, c_int, c_int32, _PTR]),
     "rgnn_halo_exchange_overlapped": (c_int, [_PTR, c_int, c_int32, _PTR]),
+    "rgnn_halo_plan_attach_grad": (c_int, [_PTR, _PTR, _PTR, _PTR, _PTR]),
+    "rgnn_halo_plan_build_reverse": (c_int, [_PTR, _PTR]),
+    "rgnn_halo_plan_num_reverse": (c_int64, [_PTR]),
+    "rgnn_halo_plan_export_reverse": (c_int, [_PTR, _PTR, _PTR, _PTR, _PTR]),
+    "rgnn_halo_exchange_backward": (c_int, [_PTR, c_int, c_int32, _PTR, _PTR, _PTR]),
     "rgnn_peer_alloc": (c_int, [ctypes.POINTER(c_void_p), c_size_t, _PTR]),
     "rgnn_peer_open": (c_int, [_PTR, ctypes.POINTER(c_void_p)]),
     "rgnn_peer_close": (c_int, [_PTR]),

@@ -13,6 +13,20 @@ reads the owners' rows over NVLink and carries its own cross-rank barrier.
         sparse_gnn_film_layer(sg.states(t % 2), sg.plan, cnt_local, d, weights=w, out=sg.states(1 - t % 2))
     result = sg.states(len(layer_weights) % 2)[:sg.n_own]
 
+Training uses the same plan and buffers in both directions: ``gather`` is differentiable, its backward is the transposed
+exchange (rgnn_halo_exchange_backward: the gradients of the halo rows are added into their owners' rows, in peer memory, in
+a fixed rank order).  The weight gradients are still summed over the ranks by the caller.
+
+    sg.attach(state_dim, training=True)          # + two gradient buffers, their flags, the published halo list;
+                                                 #   builds the reverse index on the device
+    plan = sg.training_plan()                    # GraphPlan over the device-built local lists, restricted to n_own
+    cnt = sg.local_num_incoming(type_to_num_incoming_edges)
+    h = h_own                                    # [n_own, d], e.g. a leaf that requires grad
+    for t, w in enumerate(layer_weights):
+        h = sparse_gnn_film_layer(sg.gather(h, t % 2), plan, cnt, d, weights=w)[:sg.n_own]
+    loss_of(h).backward()                        # every rank: the halo gradients travel back inside the backward pass
+    scaffold.all_reduce_gradients_(model)        # the replicated weights' gradients
+
 The reference has no multi-device path (SURVEY.md 2.1); the partition follows SURVEY.md 8(e): targets owned, sources
 fetched, weights replicated.
 """
@@ -22,10 +36,28 @@ from typing import List, Optional, Sequence
 import numpy as np
 import torch
 
-from .engine import (GraphPlan, RgnnError, RGNN_E_INVALID, c_int64, c_void_p, check, current_stream_ptr, load_library,
-                     ptr_table)
+from .engine import (GraphPlan, RgnnError, RGNN_E_INVALID, as_f32, c_int64, c_void_p, check, current_stream_ptr,
+                     load_library, ptr_table)
 
 PEER_HANDLE_BYTES = 64
+HALO_LIST_HEADER = 4          # int32 words before the owners in a published halo list (include/rgnn.h)
+
+
+class _HaloGather(torch.autograd.Function):
+    """ShardedGraph.gather: forward = the owned rows into a state buffer + rgnn_halo_exchange, returned as a fresh
+    [n_local, d] tensor; backward = rgnn_halo_exchange_backward on the gradient buffer of the same parity."""
+
+    @staticmethod
+    def forward(ctx, h_own, sg, buffer):
+        ctx.sg, ctx.buffer = sg, buffer
+        st = sg.states(buffer)
+        st[: sg.n_own].copy_(h_own)
+        sg.exchange(buffer)
+        return st.clone()
+
+    @staticmethod
+    def backward(ctx, grad_local):
+        return ctx.sg.exchange_backward(ctx.buffer, grad_local), None, None
 
 
 class _CudaView:
@@ -101,8 +133,8 @@ class ShardedGraph:
     """Rank-local structure of a node-range partition, built on the device by rgnn_halo_plan_create.
 
     ``plan`` carries no adjacency lists, so the layer paths that need them (the differentiable FiLM, RGAT, Edge-MLP,
-    RGIN and composed RGCN) refuse it with an RgnnError.  Training on a node-range partition uses a GraphPlan over
-    ``NodeRangePartition.local_adjacency_lists`` with ``set_num_targets(n_own)`` and ``NodeRangePartition.exchange``."""
+    RGIN and composed RGCN) refuse it with an RgnnError.  Training runs on ``training_plan()`` between ``gather`` calls,
+    after ``attach(state_dim, training=True)``."""
 
     def __init__(self, adjacency_lists: Sequence, cuts: Sequence[int], rank: int, world: int,
                  device: Optional[torch.device] = None, group=None):
@@ -135,6 +167,7 @@ class ShardedGraph:
                                           sum(self.local_num_edges), self.device, num_targets=self.n_own, owner=self)
         self._peer = None
         self.state_dim = None
+        self._training_plan = None
 
     @property
     def handle(self):
@@ -166,20 +199,27 @@ class ShardedGraph:
         return out
 
     # ---- peer memory -------------------------------------------------------------------------------------------
-    def attach(self, state_dim: int):
+    def attach(self, state_dim: int, training: bool = False):
         """Allocate this rank's two state buffers [n_local, state_dim] and its flag array in peer-mapped memory, exchange
-        the IPC handles (the only host-side collective) and hand the mapped pointers to the library."""
+        the IPC handles (the only host-side collective) and hand the mapped pointers to the library.
+
+        ``training=True`` also allocates, in the same peer-mapped allocation, the two gradient buffers, their own flag
+        array and this rank's published halo list (rgnn_halo_plan_attach_grad), waits for every rank to publish, and
+        builds the reverse index on the device (rgnn_halo_plan_build_reverse): ``gather`` becomes differentiable."""
         import torch.distributed as dist
         lib = load_library()
         d = int(state_dim)
         if d % 4:
             raise RgnnError(RGNN_E_INVALID, "state_dim %d must be a multiple of 4" % d)
-        rows = torch.tensor([self.n_local], dtype=torch.int64, device=self.device)
+        rows = torch.tensor([self.n_local, self.n_halo], dtype=torch.int64, device=self.device)
         if self.world > 1:
             dist.all_reduce(rows, op=dist.ReduceOp.MAX, group=self.group)
-        max_rows = int(rows.item())
+        max_rows, max_halo = (int(x) for x in rows.tolist())
         self._buf_bytes = (max_rows * d * 4 + 255) // 256 * 256          # same layout on every rank
         nbytes = 2 * self._buf_bytes + 256
+        list_bytes = ((HALO_LIST_HEADER + 2 * max_halo) * 4 + 255) // 256 * 256
+        if training:                                   # [g0][g1][gradient flags][halo list] after the forward's layout
+            nbytes += 2 * self._buf_bytes + 256 + list_bytes
         self._peer = PeerBuffer(nbytes, self.rank, self.world, self.device, self.group)
         self.state_dim = d
         s0 = (c_void_p * self.world)(*[p for p in self._peer.ptrs])
@@ -187,29 +227,122 @@ class ShardedGraph:
         fl = (c_void_p * self.world)(*[p + 2 * self._buf_bytes for p in self._peer.ptrs])
         check(lib.rgnn_halo_plan_attach(self.handle, s0, s1, fl))
         self._states = [self._peer.tensor((self.n_local, d), byte_offset=b * self._buf_bytes) for b in (0, 1)]
+        if training:
+            g0 = 2 * self._buf_bytes + 256
+            self._attach_grad([[p + g0 + b * self._buf_bytes for p in self._peer.ptrs] for b in (0, 1)],
+                              [p + g0 + 2 * self._buf_bytes for p in self._peer.ptrs],
+                              [p + g0 + 2 * self._buf_bytes + 256 for p in self._peer.ptrs])
+            if self.world > 1:
+                dist.barrier(group=self.group)        # every rank has published its halo list
+            self.build_reverse()
         return self
 
+    def _attach_grad(self, grads, flags, lists):
+        """rgnn_halo_plan_attach_grad with per-rank pointer lists (grads: one list per gradient buffer)."""
+        w = self.world
+        with torch.cuda.device(self.device):
+            check(load_library().rgnn_halo_plan_attach_grad(self.handle, (c_void_p * w)(*grads[0]), (c_void_p * w)(*grads[1]),
+                                                           (c_void_p * w)(*flags), (c_void_p * w)(*lists)))
+
     @staticmethod
-    def attach_in_process(graphs: Sequence["ShardedGraph"], state_dim: int):
+    def attach_in_process(graphs: Sequence["ShardedGraph"], state_dim: int, training: bool = False):
         """All ranks of the partition live in THIS process on one GPU ("virtual ranks": single-GPU tests of the exchange
         protocol, SURVEY.md 4.4): plain torch allocations, every rank sees every other rank's pointers directly.  The
         exchanges of the virtual ranks must then be enqueued on DIFFERENT streams (they wait for each other on the device),
         and all of their pull kernels must fit on the GPU at once (a rank's CTAs spin until every other rank's CTA 0 has run:
-        small test graphs only -- at most 264 CTAs of 512 threads per rank, 528 fit on an H100)."""
+        small test graphs only -- at most 264 CTAs of 512 threads per rank, 528 fit on an H100).  ``training=True``: as in
+        ``attach``; a training step must then make no call that waits for the device between two exchanges of a rank (the
+        other ranks' work is enqueued by the same host thread), which ``training_plan()`` arranges for the layer paths."""
         lib = load_library()
         d = int(state_dim)
         world = len(graphs)
         max_rows = max(g.n_local for g in graphs)
         buf_floats = (max_rows * d + 63) // 64 * 64
-        arenas = [torch.zeros(2 * buf_floats + 64, dtype=torch.float32, device=g.device) for g in graphs]
+        list_floats = (HALO_LIST_HEADER + 2 * max(g.n_halo for g in graphs) + 63) // 64 * 64
+        extra = 2 * buf_floats + 64 + list_floats if training else 0
+        arenas = [torch.zeros(2 * buf_floats + 64 + extra, dtype=torch.float32, device=g.device) for g in graphs]
+        base = [a.data_ptr() for a in arenas]
         for g, arena in zip(graphs, arenas):
-            base = [a.data_ptr() for a in arenas]
             s0 = (c_void_p * world)(*base)
             s1 = (c_void_p * world)(*[p + buf_floats * 4 for p in base])
             fl = (c_void_p * world)(*[p + 2 * buf_floats * 4 for p in base])
             check(lib.rgnn_halo_plan_attach(g.handle, s0, s1, fl))
             g.state_dim, g._arena, g._peer = d, arenas, "in-process"
             g._states = [arena[b * buf_floats: b * buf_floats + g.n_local * d].view(g.n_local, d) for b in (0, 1)]
+        if training:
+            for g in graphs:                          # the zeroed arenas are in place before the lists are published
+                torch.cuda.current_stream(g.device).synchronize()
+            g0 = (2 * buf_floats + 64) * 4
+            for g in graphs:
+                g._attach_grad([[p + g0 + b * buf_floats * 4 for p in base] for b in (0, 1)],
+                               [p + g0 + 2 * buf_floats * 4 for p in base],
+                               [p + g0 + (2 * buf_floats + 64) * 4 for p in base])
+            for g in graphs:
+                g.build_reverse()
+
+    def build_reverse(self):
+        """(Re)build the reverse index of the halo lists on the device (rgnn_halo_plan_build_reverse): every rank must have
+        published its list (``attach(..., training=True)`` does both).  Synchronises; refused during a CUDA-graph capture."""
+        with torch.cuda.device(self.device):
+            check(load_library().rgnn_halo_plan_build_reverse(self.handle, current_stream_ptr(self.device)))
+
+    def export_reverse(self):
+        """Copy of the reverse index (tests): offsets [n_own + 1] over the owned rows, and per entry the consuming peer and
+        the row of that peer's gradient buffer (its n_own + the halo position), sorted by (owned row, peer)."""
+        lib = load_library()
+        n = int(lib.rgnn_halo_plan_num_reverse(self.handle))
+        if n < 0:
+            raise RgnnError(RGNN_E_INVALID, "the reverse index has not been built (attach(state_dim, training=True))")
+        out = {"offsets": torch.empty(self.n_own + 1, dtype=torch.int32, device=self.device),
+               "peer": torch.empty(max(n, 1), dtype=torch.int32, device=self.device),
+               "row": torch.empty(max(n, 1), dtype=torch.int32, device=self.device)}
+        with torch.cuda.device(self.device):
+            check(lib.rgnn_halo_plan_export_reverse(self.handle, out["offsets"].data_ptr(), out["peer"].data_ptr(),
+                                                    out["row"].data_ptr(), current_stream_ptr(self.device)))
+        out["peer"], out["row"] = out["peer"][:n], out["row"][:n]
+        return out
+
+    def training_plan(self) -> GraphPlan:
+        """The plan the differentiable layer paths run on between ``gather`` calls: a GraphPlan over this rank's
+        device-exported local adjacency lists, restricted to the owned rows.  Built once; its index views and regrouped
+        plans are built here, eagerly, so that a training step neither synchronises nor builds plan state inside a
+        CUDA-graph capture."""
+        if self._training_plan is None:
+            lists = self.export()["local_adjacency_lists"]
+            plan = GraphPlan(lists, self.n_local, device=self.device).set_num_targets(self.n_own)
+            for view in ("message_sources", "message_targets", "message_types", "in_degree"):
+                getattr(plan, view)
+            for by in ("source", "source_type", "target_type"):
+                plan.regrouped(by)
+            self._training_plan = plan
+        return self._training_plan
+
+    def gather(self, h_own: torch.Tensor, buffer: int) -> torch.Tensor:
+        """[n_own, state_dim] owned states -> a fresh [n_local, state_dim] tensor: owned rows, then the halo rows pulled
+        from their owners through state buffer ``buffer`` (rgnn_halo_exchange).  Collective.  Differentiable: the backward
+        adds the gradients of the halo rows into their owners' rows (rgnn_halo_exchange_backward, gradient buffer
+        ``buffer``), which needs ``attach(..., training=True)``.  Consecutive gathers alternate the buffer, and every rank
+        runs the backward of each gather (a rank that skips one leaves its peers waiting)."""
+        d = self.state_dim or 0
+        if not isinstance(h_own, torch.Tensor) or tuple(h_own.shape) != (self.n_own, d):
+            raise RgnnError(RGNN_E_INVALID, "gather: h_own must be [n_own, state_dim] = [%d, %d], got %s"
+                            % (self.n_own, d, tuple(getattr(h_own, "shape", ()))))
+        return _HaloGather.apply(as_f32(h_own, "h_own"), self, int(buffer))
+
+    def exchange_backward(self, buffer: int, grad_local: torch.Tensor) -> torch.Tensor:
+        """The transposed exchange (rgnn_halo_exchange_backward): [n_local, state_dim] local gradient -> [n_own,
+        state_dim] = its owned rows plus, per row, the gradients the peers hold for it as a halo row, added in ascending
+        rank.  Collective."""
+        d = self.state_dim or 0
+        g = as_f32(grad_local, "grad_local")
+        if tuple(g.shape) != (self.n_local, d):
+            raise RgnnError(RGNN_E_INVALID, "exchange_backward: grad_local must be [n_local, state_dim] = [%d, %d], got %s"
+                            % (self.n_local, d, tuple(g.shape)))
+        out = torch.empty((self.n_own, d), dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            check(load_library().rgnn_halo_exchange_backward(self.handle, int(buffer), d, g.data_ptr(), out.data_ptr(),
+                                                             current_stream_ptr(self.device)))
+        return out
 
     def states(self, buffer: int) -> torch.Tensor:
         """This rank's state buffer 0 / 1 as a [n_local, state_dim] tensor (owned rows first, then the halo rows)."""
@@ -232,6 +365,9 @@ class ShardedGraph:
     def close(self):
         if getattr(self, "_handle", None) is not None:
             torch.cuda.synchronize(self.device)
+            if self._training_plan is not None:
+                self._training_plan.close()
+                self._training_plan = None
             self._states = None
             if self._peer is not None and not isinstance(self._peer, str):
                 if self.world > 1:
