@@ -7,7 +7,7 @@ for the persistent wgmma GEMM, whose CTAs walk several tiles once there are more
 a single split of the TN weight-gradient GEMM at >= 132 output tiles.  Each case below is sized just past the threshold it
 targets.  Its regime is restated from the case parameters (checked without a GPU by test_case_regimes) and the kernel the
 regime implies must appear among the launched kernels, so a changed heuristic fails here instead of silently testing the
-small-batch path again.  No RGNN_* environment variable is set: these are the default dispatch paths."""
+small-batch path again."""
 import zlib
 
 import numpy as np

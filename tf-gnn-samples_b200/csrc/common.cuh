@@ -119,8 +119,7 @@ static inline cudaError_t launch_pdl(void (*kernel)(Params), dim3 grid, dim3 blo
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
-  static const bool off = getenv("RGNN_NO_PDL") != nullptr;   // A/B knob: plain stream-ordered launches
-  cfg.attrs = attr; cfg.numAttrs = off ? 0 : 1;
+  cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, params);
 }
 

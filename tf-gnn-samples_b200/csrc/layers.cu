@@ -373,7 +373,7 @@ extern "C" int rgnn_rgcn_forward(const rgnn_plan_t* plan, const float* h, int32_
 //   d_agg = grad_out * act'(.) / div            (elementwise)
 //   d_T[u, l, :] = sum_{(u->v) in A_l} s_{l,v} * d_agg[v, :]      (sorted-segment kernel over the reverse index)
 //   d_H = d_T . [W_0|...|W_{L-1}]^T             (wgmma GEMM, transposed weight images)
-//   d_W_l = H^T . d_T[:, l, :]                  (tiled FMA kernel, deterministic two-stage sum)
+//   d_W_l = H^T . d_T[:, l, :]                  (TN wgmma GEMM, split-K with a deterministic two-stage sum)
 extern "C" int rgnn_rgcn_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d_in, int32_t d_out,
                                   const float* const* edge_weights, const float* num_incoming, int activation,
                                   int aggregation, int normalize, const float* out, const float* grad_out,
@@ -402,9 +402,8 @@ extern "C" int rgnn_rgcn_backward(const rgnn_plan_t* plan_c, const float* h, int
     pre = ar.floats((size_t)V * d_out);
     t_fwd = ar.floats((size_t)V * L * d_out);
   }
-  static const bool gradw_fma = getenv("RGNN_GRADW_IMPL") != nullptr && strcmp(getenv("RGNN_GRADW_IMPL"), "fma") == 0;   // A/B reference
   float* gw_scratch = nullptr;
-  if (grad_edge_weights) gw_scratch = ar.floats(gradw_fma ? grad_weight_scratch_floats(V, L, d_in, d_out) : gemm_tn_scratch_floats(d_in, L * d_out, V));
+  if (grad_edge_weights) gw_scratch = ar.floats(gemm_tn_scratch_floats(d_in, L * d_out, V));
   RGNN_PROPAGATE(check_ws(ar, "rgcn_backward"));
 
   if (pre != nullptr) {
@@ -438,16 +437,13 @@ extern "C" int rgnn_rgcn_backward(const rgnn_plan_t* plan_c, const float* h, int
   }
   if (grad_edge_weights != nullptr) {
     // dW_l = H^T . dT[:, l, :]  -- one TN contraction over the V nodes for all types (gemm_tn_wgmma.cu)
-    GradWTable tab;
     GemmTnOut tn;
     tn.block_cols = d_out; tn.ld = d_out;
     for (int l = 0; l < L; ++l) {
       RGNN_REQUIRE(grad_edge_weights[l] != nullptr && aligned16(grad_edge_weights[l]), "rgcn_backward: grad weight %d is NULL / misaligned", l);
-      tab.out[l] = grad_edge_weights[l];
       tn.ptr[l] = grad_edge_weights[l];
     }
-    if (gradw_fma) RGNN_PROPAGATE(launch_grad_weights(h, d_t, V, L, d_in, d_out, tab, gw_scratch, stream));
-    else RGNN_PROPAGATE(launch_gemm_tn(h, d_in, d_t, L * d_out, d_in, L * d_out, V, tn, gw_scratch, stream));
+    RGNN_PROPAGATE(launch_gemm_tn(h, d_in, d_t, L * d_out, d_in, L * d_out, V, tn, gw_scratch, stream));
   }
   return RGNN_OK;
 }
@@ -552,9 +548,8 @@ extern "C" int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* h, int32_
   Arena ar(workspace, workspace_bytes);
   float* T = ar.floats((size_t)V * L * D);
   float* m = ar.floats((size_t)V * D);
-  static const int slab_env = getenv("RGNN_GRU_SLAB") ? atoi(getenv("RGNN_GRU_SLAB")) : 0;   // rows per slab (experiment knob)
-  const int slab_default = RGNN_WAVE_SMS * 128;                               // one wave of 128-row tiles
-  const int slab = slab_env > 0 ? slab_env : (V < slab_default ? (V > 0 ? V : 1) : slab_default);
+  const int slab_max = RGNN_WAVE_SMS * 128;                                   // GRU rows per slab: one wave of 128-row tiles
+  const int slab = V < slab_max ? (V > 0 ? V : 1) : slab_max;
   float* z = ar.floats((size_t)slab * D);
   float* rh = ar.floats((size_t)slab * D);
   float* buf[2] = {ar.floats((size_t)V * D), ar.floats((size_t)V * D)};
@@ -570,12 +565,7 @@ extern "C" int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* h, int32_
     s.D = D;
     RGNN_PROPAGATE(transform_sources(plan, ar, cur, D, D, edge_weights, T, stream, s));   // ggnn.py:80-82
     s.agg = aggregation; s.out = m; s.ld_out = D; s.heavy_scratch = heavy.heavy_scratch;   // ggnn.py:87-90
-    // Experiment (RGNN_GRU_SLAB_EDGES=1; needs a batch without heavy targets): slab the edge stage together with the cell so
-    // that a slab's aggregated messages are consumed out of L2.  Measured on QM9-10k: 1.975 ms vs 1.928 ms without (job L) --
-    // five small edge-stage launches cost more than the saved round trip of m; off by default.
-    static const bool slab_edges_env = getenv("RGNN_GRU_SLAB_EDGES") != nullptr && atoi(getenv("RGNN_GRU_SLAB_EDGES")) == 1;
-    const bool slab_edges = slab_edges_env && cell_kind == RGNN_CELL_GRU && plan->num_heavy_host == 0;
-    if (!slab_edges) RGNN_PROPAGATE(launch_seg_reduce(s, stream));
+    RGNN_PROPAGATE(launch_seg_reduce(s, stream));
     GemmParams g;
     g.A1 = m; g.lda1 = D; g.K1 = D;
     g.M = plan->Vt; g.bias = cell_bias;   // the cell runs on the wanted target rows only
@@ -593,22 +583,15 @@ extern "C" int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* h, int32_
       for (int r0 = 0; r0 < Vc; r0 += slab) {
         const int rows = (Vc - r0 < slab) ? Vc - r0 : slab;
         const size_t off = (size_t)r0 * D;
-        const float* m_slab = m + off;
-        if (slab_edges) {                                  // aggregate this slab's targets into the first rows of m (reused by every slab)
-          SegParams q = s;
-          q.V = rows; q.seg_off = s.seg_off + r0; q.out = m;
-          RGNN_PROPAGATE(launch_seg_reduce(q, stream));
-          m_slab = m;
-        }
         GemmParams g2 = g;
-        g2.A1 = m_slab; g2.M = rows;
+        g2.A1 = m + off; g2.M = rows;
         g2.A2 = cur + off; g2.lda2 = D; g2.K2 = D;
         g2.B1 = cell_kernel; g2.ldb1 = 3 * D; g2.B2 = cell_recurrent_kernel; g2.ldb2 = 3 * D;
         g2.N = 2 * D; g2.C = z; g2.ldc = D; g2.C2 = rh; g2.ldc2 = D; g2.aux_h = cur + off; g2.ld_h = D;
         g2.epi = EPI_GRU_ZR;
         RGNN_PROPAGATE(run_gemm(g2, ar, stream));
         GemmParams o;
-        o.A1 = m_slab; o.lda1 = D; o.K1 = D; o.A2 = rh; o.lda2 = D; o.K2 = D;
+        o.A1 = m + off; o.lda1 = D; o.K1 = D; o.A2 = rh; o.lda2 = D; o.K2 = D;
         o.B1 = cell_kernel + 2 * D; o.ldb1 = 3 * D; o.B2 = cell_recurrent_kernel + 2 * D; o.ldb2 = 3 * D;
         o.M = rows; o.N = D; o.bias = cell_bias + 2 * D; o.C = dst + off; o.ldc = D;
         o.aux_h = cur + off; o.ld_h = D; o.aux_z = z; o.ld_z = D;
@@ -644,7 +627,7 @@ extern "C" int rgnn_rgat_forward(const rgnn_plan_t* plan, const float* h, int32_
   float* T = ar.floats((size_t)V * L * D);
   // per-edge logits: computed inside the edge kernel when a head's dh/4 lanes form a power-of-two group inside one warp
   const int dh = D / K, lph = dh / 4;
-  const bool fused_scores = (dh % 4) == 0 && lph >= 1 && lph <= 32 && (lph & (lph - 1)) == 0 && getenv("RGNN_RGAT_UNFUSED") == nullptr;
+  const bool fused_scores = (dh % 4) == 0 && lph >= 1 && lph <= 32 && (lph & (lph - 1)) == 0;
   float* ssrc = fused_scores ? nullptr : ar.floats((size_t)V * L * K);
   float* stgt = fused_scores ? nullptr : ar.floats((size_t)V * L * K);
   float* buf[2] = {nullptr, nullptr};
@@ -697,42 +680,22 @@ extern "C" int rgnn_film_forward(const rgnn_plan_t* plan, const float* h, int32_
   int din = d_in;
   for (int t = 0; t < num_timesteps; ++t) {                                   // gnn_film.py:85
     float* dst = (t == num_timesteps - 1) ? out : buf[t & 1];
-    // [gamma | beta] = F_l h_v for the wanted target rows (:102).  Experiment (RGNN_FILM_SLAB=1; plans without heavy targets):
-    // row slabs small enough (<= 48 MB of gamma / beta rows) that the edge stage reads them back out of L2, target-side GEMM
-    // and edge stage alternating per slab.  Measured on config 5 (50k / 1M): 0.441 ms vs 0.343 ms with ONE slab (job L) -- the
-    // seven short GEMM / edge-stage launch pairs lose more to tails than L2 residency returns; off by default.
-    const int Vc = plan->Vt;
-    int slab = Vc > 0 ? Vc : 1;
-    static const bool film_slab_env = getenv("RGNN_FILM_SLAB") != nullptr && atoi(getenv("RGNN_FILM_SLAB")) == 1;
-    if (film_slab_env && plan->num_heavy_host == 0) {
-      const long rows_fit = (48L << 20) / ((long)L * 2 * D * (long)sizeof(float));
-      const long r = rows_fit / 128 * 128;
-      if (r >= 1024 && r < slab) slab = (int)r;
-    }
-    // One slab (the default): the target-side GEMM goes FIRST -- it reads owned rows only, so on a sharded plan it overlaps a
-    // pending halo exchange (rgnn_halo_exchange_overlapped), which transform_sources() below joins before touching halo rows.
-    const bool fw_first = slab >= Vc;
-    if (fw_first && Vc > 0)
-      RGNN_PROPAGATE(gemm_shared_a(ar, cur, Vc, din, film_weights, L, 2 * D, 2 * D, FW, RGNN_ACT_LINEAR, stream));
+    // [gamma | beta] = F_l h_v for the wanted target rows (:102).  This GEMM goes FIRST: it reads owned rows only, so on a
+    // sharded plan it overlaps a pending halo exchange (rgnn_halo_exchange_overlapped), which transform_sources() below joins
+    // before touching halo rows.
+    if (plan->Vt > 0)
+      RGNN_PROPAGATE(gemm_shared_a(ar, cur, plan->Vt, din, film_weights, L, 2 * D, 2 * D, FW, RGNN_ACT_LINEAR, stream));
     SegParams s;
     seg_from_plan(s, plan);
     s.D = D;
     RGNN_PROPAGATE(transform_sources(plan, ar, cur, din, D, edge_weights, T, stream, s));                        // :94 on nodes
     s.num_incoming = normalize ? num_incoming : nullptr;                      // :96-100
-    s.msg_mode = MSG_FILM; s.mod_stride_node = (long)L * 2 * D; s.mod_stride_type = 2 * D;                        // :103-108
+    s.msg_mode = MSG_FILM; s.mod_table = FW; s.mod_stride_node = (long)L * 2 * D; s.mod_stride_type = 2 * D;      // :103-108
     s.act_msg = activation;                                                   // :112 (before the sum)
     s.agg = aggregation;                                                      // :113-116
     s.ln_gamma = ln_gamma + (size_t)t * D; s.ln_beta = ln_beta + (size_t)t * D;   // :120
-    s.ld_out = D; s.heavy_scratch = heavy.heavy_scratch;
-    for (int r0 = 0; r0 < Vc; r0 += slab) {
-      const int rows = (Vc - r0 < slab) ? Vc - r0 : slab;
-      if (!fw_first) RGNN_PROPAGATE(gemm_shared_a(ar, cur + (size_t)r0 * din, rows, din, film_weights, L, 2 * D, 2 * D, FW, RGNN_ACT_LINEAR, stream));
-      SegParams q = s;
-      q.V = rows; q.seg_off = s.seg_off + r0; q.mod_table = FW;             // FW holds this slab's rows from row 0
-      if (q.num_incoming != nullptr) q.num_incoming = s.num_incoming + r0;    // c[type, v] = base[type * ld + v]
-      q.out = dst + (size_t)r0 * D;
-      RGNN_PROPAGATE(launch_seg_reduce(q, stream));
-    }
+    s.out = dst; s.ld_out = D; s.heavy_scratch = heavy.heavy_scratch;
+    RGNN_PROPAGATE(launch_seg_reduce(s, stream));
     cur = dst; din = D;
   }
   return RGNN_OK;

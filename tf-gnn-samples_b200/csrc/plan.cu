@@ -386,7 +386,7 @@ extern "C" int rgnn_plan_create_ex(rgnn_plan_t** out, int32_t num_nodes, int32_t
   }
   // compact (source, type) pair table for sparsely typed graphs (see plan.cuh)
   const size_t VL = (size_t)num_nodes * num_edge_types;
-  if ((double)M < 0.75 * (double)VL && getenv("RGNN_NO_PAIRS") == nullptr) {
+  if ((double)M < 0.75 * (double)VL) {
     const size_t rank_bytes = align_up(sizeof(int32_t) * (VL + 1), 256);
     size_t scan_bytes = 0;
     PLAN_CUDA2(cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, (const int32_t*)nullptr, (int32_t*)nullptr, (int)(VL + 1), stream));

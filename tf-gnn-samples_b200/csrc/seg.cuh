@@ -108,10 +108,4 @@ int launch_layer_norm(const float* x, int rows, int D, const float* gamma, const
 int launch_act_backward(const float* grad_out, const float* out, const float* pre, int V, int D, int act, int agg,
                         const int32_t* seg_off, float* d_agg, cudaStream_t stream);
 
-// grad_w[l][i][j] = sum_v h[v, i] * d_t[v, l, j]   (d_t is [V, L, D], h is [V, Din]); deterministic two-stage sum.
-struct GradWTable { float* out[RGNN_MAX_EDGE_TYPES]; };
-size_t grad_weight_scratch_floats(int V, int L, int d_in, int d_out);
-int launch_grad_weights(const float* h, const float* d_t, int V, int L, int d_in, int d_out, const GradWTable& out,
-                        float* scratch, cudaStream_t stream);
-
 }  // namespace rgnn

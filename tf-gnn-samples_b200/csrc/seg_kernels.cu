@@ -13,8 +13,6 @@
 // (rgat.py:120-138), tf.contrib.layers.layer_norm (A.5).
 #include "seg.cuh"
 
-#include <stdlib.h>
-
 namespace rgnn {
 
 namespace {
@@ -248,86 +246,6 @@ __global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_half_kernel(c
   bool ok1[1] = {okc && half == 0};
   float4 a1[1] = {acc};
   seg_finish<1>(p, v, col0, lane, ok1, end - beg, a1);
-}
-
-// EXPERIMENT (RGNN_SEG_BULK=1; VERDICT r1 item 6: "measure a cp.async.bulk row-gather variant once"): the north star's
-// sketch -- rows pulled into shared memory by the TMA unit -- for the plain edge stage (linear messages, sum / mean / sqrt_n).
-// A warp owns a 128-column slice of one target; lane 0 issues one 512-byte cp.async.bulk per gathered row into the warp's own
-// ring (2 batches x 5 rows), completion on an mbarrier per batch; the lanes then read their float4 of every landed row from
-// shared memory and accumulate.  One bulk-copy instruction per row instead of 32 LDG.128 lanes, but every gathered byte is
-// written to and read back from shared memory once more.  Result: see DESIGN.md 5.2 / profiles/r02_seg_bulk.txt.
-constexpr int BULK_ROWS = 5;   // 8 warps x 2 batches x 5 rows x 512 B = 40 KB of static shared memory
-template <bool SCALED>
-__global__ void __launch_bounds__(WARPS_PER_BLOCK * 32) seg_reduce_bulk_kernel(const __grid_constant__ SegParams p) {
-  __shared__ __align__(128) float ring[WARPS_PER_BLOCK][2][BULK_ROWS][128];
-  __shared__ __align__(8) unsigned long long bars[WARPS_PER_BLOCK][2];
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  const int v = blockIdx.x * WARPS_PER_BLOCK + w;
-  const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(&bars[w][0]), bar1 = (uint32_t)__cvta_generic_to_shared(&bars[w][1]);
-  if (lane == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar0));
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar1));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncwarp();
-  if (v >= p.V) return;
-  const int col0 = blockIdx.y * 128;                     // slice start; the slice is 128 columns (512 bytes) wide
-  const int width = min(128, p.D - col0);                // D % 4 == 0; bulk copies need multiples of 16 bytes
-  const int beg = __ldg(p.seg_off + v), end = __ldg(p.seg_off + v + 1);
-  pdl_wait();
-  pdl_launch_dependents();
-  if (p.heavy_threshold > 0 && end - beg > p.heavy_threshold) return;
-  float4 acc = f4(0.0f);
-  const bool okc = lane * 4 < width;
-  const int nb = (end - beg + BULK_ROWS - 1) / BULK_ROWS;
-  auto issue = [&](int b) {                              // batch b: edges [beg + 8b, +8) -> ring slot b & 1
-    const int e0 = beg + b * BULK_ROWS;
-    const int n = min(BULK_ROWS, end - e0);
-    float sc = 1.0f;
-    long off = 0;
-    if (lane < n) {
-      const int ty = __ldg(p.e_type + e0 + lane), idx = __ldg(p.e_idx + e0 + lane);
-      off = (long)idx * p.stride_idx + (long)ty * p.stride_type + col0;
-      if (SCALED) sc = 1.0f / (__ldg(p.num_incoming + (size_t)ty * p.scale_ld + (p.scale_by_idx ? idx : v)) + 1e-7f);
-    }
-    const uint32_t bar = (b & 1) ? bar1 : bar0;
-    if (lane == 0) asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"((uint32_t)(n * width * 4)) : "memory");
-    __syncwarp();
-    if (lane < n) {
-      const uint32_t dst = (uint32_t)__cvta_generic_to_shared(&ring[w][b & 1][lane][0]);
-      asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                   ::"r"(dst), "l"(p.table + off), "r"((uint32_t)(width * 4)), "r"(bar) : "memory");
-    }
-    return sc;
-  };
-  float sc_cur = 0.0f, sc_next = 0.0f;
-  if (nb > 0) sc_cur = issue(0);
-  for (int b = 0; b < nb; ++b) {
-    if (b + 1 < nb) sc_next = issue(b + 1);
-    const uint32_t bar = (b & 1) ? bar1 : bar0;
-    const uint32_t parity = (uint32_t)((b >> 1) & 1);
-    uint32_t ok = 0, spins = 0;
-    while (!ok) {
-      asm volatile("{\n\t.reg .pred q;\n\tmbarrier.try_wait.parity.shared::cta.b64 q, [%1], %2;\n\tselp.u32 %0, 1, 0, q;\n\t}"
-                   : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
-      if (++spins > (1u << 22)) __trap();
-    }
-    const int n = min(BULK_ROWS, end - (beg + b * BULK_ROWS));
-#pragma unroll
-    for (int r = 0; r < BULK_ROWS; ++r) {
-      const float s_r = __shfl_sync(0xffffffffu, sc_cur, r);
-      if (r < n && okc) {
-        const float4 m = *reinterpret_cast<const float4*>(&ring[w][b & 1][r][lane * 4]);
-        if (SCALED) { acc.x = fmaf(m.x, s_r, acc.x); acc.y = fmaf(m.y, s_r, acc.y); acc.z = fmaf(m.z, s_r, acc.z); acc.w = fmaf(m.w, s_r, acc.w); }
-        else acc = add4(acc, m);
-      }
-    }
-    __syncwarp();                                        // every lane has read slot b & 1 before batch b + 2 overwrites it
-    sc_cur = sc_next;
-  }
-  bool ok1[1] = {okc};
-  float4 a1[1] = {acc};
-  seg_finish<1>(p, v, col0 + lane * 4, lane, ok1, end - beg, a1);
 }
 
 // Degree skew: a target with thousands of incoming edges would serialise on one warp (Zipf-skewed PPI-shaped
@@ -839,110 +757,40 @@ __global__ void act_backward_kernel(const float* __restrict__ grad_out, const fl
   *reinterpret_cast<float4*>(d_agg + i * 4) = make_float4(g.x * d.x * inv, g.y * d.y * inv, g.z * d.z * inv, g.w * d.w * inv);
 }
 
-// grad_w partials: CTA = 64 x 64 tile of one type's [Din, D] gradient over one slice of the node range.
-constexpr int GW_TILE = 64, GW_ROWS = 32;
-__global__ void __launch_bounds__(256) grad_weight_partial_kernel(const float* __restrict__ h, const float* __restrict__ d_t,
-                                                                 int V, int L, int d_in, int d_out, int splits,
-                                                                 float* __restrict__ partial) {
-  __shared__ float hs[GW_ROWS][GW_TILE + 4];
-  __shared__ float ts[GW_ROWS][GW_TILE + 4];
-  const int l = blockIdx.z / splits, sp = blockIdx.z % splits;
-  const int i0 = blockIdx.y * GW_TILE, j0 = blockIdx.x * GW_TILE;
-  const int rows_per = (V + splits - 1) / splits;
-  const int v0 = sp * rows_per, v1 = min(V, v0 + rows_per);
-  const int tx = threadIdx.x & 15, ty = threadIdx.x >> 4;
-  float acc[4][4] = {};
-  for (int vb = v0; vb < v1; vb += GW_ROWS) {
-    for (int f = threadIdx.x; f < GW_ROWS * (GW_TILE / 4); f += 256) {
-      const int r = f / (GW_TILE / 4), c4 = (f % (GW_TILE / 4)) * 4;
-      const int v = vb + r;
-      float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-      if (v < v1) {
-        if (i0 + c4 < d_in) a = ldg4(h + (size_t)v * d_in + i0 + c4);
-        if (j0 + c4 < d_out) b = ldg4(d_t + ((size_t)v * L + l) * d_out + j0 + c4);
-      }
-      *reinterpret_cast<float4*>(&hs[r][c4]) = a;
-      *reinterpret_cast<float4*>(&ts[r][c4]) = b;
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int r = 0; r < GW_ROWS; ++r) {
-      const float4 a = *reinterpret_cast<const float4*>(&hs[r][ty * 4]);
-      const float4 b = *reinterpret_cast<const float4*>(&ts[r][tx * 4]);
-      const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-      for (int x = 0; x < 4; ++x)
-#pragma unroll
-        for (int y = 0; y < 4; ++y) acc[x][y] = fmaf(av[x], bv[y], acc[x][y]);
-    }
-    __syncthreads();
-  }
-  float* dst = partial + ((size_t)(sp * L + l) * d_in) * d_out;
-#pragma unroll
-  for (int x = 0; x < 4; ++x) {
-    const int i = i0 + ty * 4 + x;
-    if (i < d_in && j0 + tx * 4 < d_out)
-      *reinterpret_cast<float4*>(dst + (size_t)i * d_out + j0 + tx * 4) = make_float4(acc[x][0], acc[x][1], acc[x][2], acc[x][3]);
-  }
-}
-
-__global__ void grad_weight_reduce_kernel(const float* __restrict__ partial, int L, int d_in, int d_out, int splits,
-                                          const __grid_constant__ GradWTable out) {
-  const long per_type = (long)d_in * d_out / 4;
-  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= per_type * L) return;
-  const int l = (int)(i / per_type);
-  const long e = (i % per_type) * 4;
-  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int sp = 0; sp < splits; ++sp) {   // fixed order: deterministic
-    const float4 x = ldg4(partial + ((size_t)(sp * L + l) * d_in) * d_out + e);
-    s.x += x.x; s.y += x.y; s.z += x.z; s.w += x.w;
-  }
-  *reinterpret_cast<float4*>(out.out[l] + e) = s;
-}
-
-inline int grad_weight_splits(int V, int L, int d_in, int d_out) {
-  const int tiles = ((d_in + GW_TILE - 1) / GW_TILE) * ((d_out + GW_TILE - 1) / GW_TILE) * L;
-  int splits = (2 * RGNN_WAVE_SMS + tiles - 1) / tiles;
-  const int max_by_rows = (V + 63) / 64;
-  if (splits > max_by_rows) splits = max_by_rows;
-  if (splits > 64) splits = 64;
-  if (splits < 1) splits = 1;
-  return splits;
-}
-
 inline int nv_for(int D) { return (D + 127) / 128; }
 
 }  // namespace
 
-static int seg_cols() {   // experiment knob: RGNN_SEG_COLS=256 -> one warp per 256-column slice (default 128)
-  static int c = -1;
-  if (c < 0) {
-    const char* e = getenv("RGNN_SEG_COLS");
-    c = e ? atoi(e) : 128;
-    if (c != 128 && c != 256) c = 128;
+// Targets with more than heavy_threshold incoming edges, which the warp-per-target kernels skip.  When the plan is KNOWN to
+// hold heavy targets and has scratch: the multi-CTA split (partial rows per work item, then one warp per target).  Otherwise,
+// unless the plan is known to hold none, a few persistent CTAs of the one-CTA-per-target kernel walk the heavy list; with an
+// unread count (deferred validation) that list is usually empty.  grid_y = number of 128*NV-column slices.
+template <int NV, int MODE, bool MAXAGG, bool SCALED, bool ACTMSG>
+static void launch_seg_heavy(const SegParams& p, unsigned grid_y, cudaStream_t stream) {
+  if (p.heavy_threshold <= 0 || p.heavy_known == 0) return;
+  if (p.heavy_known > 0 && p.heavy_scratch != nullptr && p.heavy_items != nullptr) {
+    const unsigned ix = p.heavy_items_known > 0 ? (unsigned)(p.heavy_items_known < 1184 ? p.heavy_items_known : 1184) : 296u;
+    seg_reduce_heavy_part_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG><<<dim3(ix, grid_y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
+    const unsigned fx = (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK);
+    seg_reduce_heavy_finish_kernel<NV, MAXAGG><<<dim3(fx, grid_y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
+    count_launch(2);
+    return;
   }
-  return c;
+  const unsigned gx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
+  seg_reduce_heavy_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG><<<dim3(gx, grid_y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
+  count_launch();
 }
 template <int NV, int MODE, bool MAXAGG, bool SCALED, bool ACTMSG>
 static void launch_seg_pair(const SegParams& p, dim3 grid, cudaStream_t stream) {
   launch_pdl(seg_reduce_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p);
   count_launch();
-  if (p.heavy_threshold > 0 && p.heavy_known != 0) {   // unknown (-1) or > 0: a few persistent CTAs walk the heavy list
-    // multi-CTA split (partial rows per work item, then one warp per target) when the plan is KNOWN to hold heavy targets; with
-    // an unread count (deferred validation) one launch of the one-CTA-per-target kernel walks the -- usually empty -- list
-    if (p.heavy_known > 0 && p.heavy_scratch != nullptr && p.heavy_items != nullptr) {
-      const unsigned ix = p.heavy_items_known > 0 ? (unsigned)(p.heavy_items_known < 1184 ? p.heavy_items_known : 1184) : 296u;
-      seg_reduce_heavy_part_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG><<<dim3(ix, grid.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-      const unsigned fx = p.heavy_known > 0 ? (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK) : (unsigned)RGNN_WAVE_SMS;
-      seg_reduce_heavy_finish_kernel<NV, MAXAGG><<<dim3(fx, grid.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-      count_launch(2);
-      return;
-    }
-    const unsigned gx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
-    seg_reduce_heavy_kernel<NV, MODE, MAXAGG, SCALED, ACTMSG><<<dim3(gx, grid.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-    count_launch();
-  }
+  launch_seg_heavy<NV, MODE, MAXAGG, SCALED, ACTMSG>(p, grid.y, stream);
+}
+template <bool SCALED>
+static void launch_seg_half(const SegParams& p, unsigned gx, cudaStream_t stream) {
+  launch_pdl(seg_reduce_half_kernel<SCALED>, dim3(gx, (p.D + 63) / 64), dim3(WARPS_PER_BLOCK * 32), 0, stream, p);
+  count_launch();
+  launch_seg_heavy<1, MSG_LINEAR, false, SCALED, false>(p, (p.D + 127) / 128, stream);
 }
 template <int NV, int MODE, bool MAXAGG, bool SCALED>
 static void launch_seg_act(const SegParams& p, dim3 grid, cudaStream_t stream) {
@@ -984,8 +832,7 @@ int launch_seg_reduce(const SegParams& p, cudaStream_t stream) {
     // Small batches: one warp per WHOLE row leaves too few warps to hide the gather latency (PPI-shaped Edge-MLP0: 2,245
     // warps, 73 us).  Reduce with one warp per 128-column slice instead and normalise the finished rows in a second, tiny
     // pass (V x D x 8 bytes; the layer-norm kernel works in place: it holds the row in registers).
-    static const int ln_split_env = getenv("RGNN_LN_SPLIT") ? atoi(getenv("RGNN_LN_SPLIT")) : -1;   // 0 / 1 force
-    const bool ln_split = p.D > 128 && p.ld_out == p.D && (ln_split_env == 1 || (ln_split_env != 0 && (long)p.V < (long)RGNN_WAVE_SMS * 40));
+    const bool ln_split = p.D > 128 && p.ld_out == p.D && (long)p.V < (long)RGNN_WAVE_SMS * 40;
     if (ln_split) {
       SegParams q = p;
       q.ln_gamma = nullptr; q.ln_beta = nullptr;
@@ -1000,49 +847,14 @@ int launch_seg_reduce(const SegParams& p, cudaStream_t stream) {
       case 3: launch_seg_nv<3>(p, grid, stream); break;
       default: launch_seg_nv<4>(p, grid, stream); break;
     }
-  } else {                       // otherwise one warp per <= 256-column slice of a target row
-    RGNN_REQUIRE(p.stride_type == 0 || (p.stride_idx % p.stride_type) == 0, "segment reduce: stride_idx must be a multiple of stride_type");
-    // one warp per 128-column slice: measured 2.2x faster than whole-row warps at D=256 (the loop is
-    // latency-bound, more independent warps win: profiles/r01_seg_reduce_v3.txt)
-    // small problems: twice as many warps, two edges per load instruction (seg_reduce_half_kernel)
-    static const int half_env = getenv("RGNN_SEG_HALF") ? atoi(getenv("RGNN_SEG_HALF")) : -1;   // 0 / 1 force, default auto
+  } else {
+    // One warp per 128-column slice: measured 2.2x faster than whole-row warps at D = 256 (the loop is latency-bound, more
+    // independent warps win).  Small problems: twice as many warps, two edges per load instruction (seg_reduce_half_kernel).
     const long warps128 = (long)p.V * ((p.D + 127) / 128);
-    const bool half_ok = p.msg_mode == MSG_LINEAR && p.agg != RGNN_AGG_MAX && p.act_msg == RGNN_ACT_LINEAR && p.D >= 64;
-    const bool use_half = half_ok && (half_env == 1 || (half_env != 0 && warps128 < (long)RGNN_WAVE_SMS * 40));
-    static const bool bulk_env = getenv("RGNN_SEG_BULK") != nullptr && atoi(getenv("RGNN_SEG_BULK")) == 1;   // experiment: TMA row gather
-    if (bulk_env && half_ok && (p.stride_idx % 4) == 0) {
-      const dim3 grid(gx, (p.D + 127) / 128);
-      if (p.num_incoming != nullptr) RGNN_CHECK_CUDA(launch_pdl(seg_reduce_bulk_kernel<true>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));
-      else RGNN_CHECK_CUDA(launch_pdl(seg_reduce_bulk_kernel<false>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));
-      count_launch();
-      if (p.heavy_threshold > 0 && p.heavy_known != 0) {
-        const unsigned hx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
-        const dim3 hgrid(hx, (p.D + 127) / 128);
-        if (p.num_incoming != nullptr) seg_reduce_heavy_kernel<1, MSG_LINEAR, false, true, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        else seg_reduce_heavy_kernel<1, MSG_LINEAR, false, false, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        count_launch();
-      }
-    } else if (use_half) {
-      const dim3 grid(gx, (p.D + 63) / 64);
-      if (p.num_incoming != nullptr) launch_pdl(seg_reduce_half_kernel<true>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p);
-      else launch_pdl(seg_reduce_half_kernel<false>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p);
-      count_launch();
-      if (p.heavy_threshold > 0 && p.heavy_known > 0 && p.heavy_scratch != nullptr && p.heavy_items != nullptr) {
-        const dim3 g128(1, (p.D + 127) / 128);
-        const unsigned ix = p.heavy_items_known > 0 ? (unsigned)(p.heavy_items_known < 1184 ? p.heavy_items_known : 1184) : 296u;
-        const unsigned fx = p.heavy_known > 0 ? (unsigned)((p.heavy_known + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK) : (unsigned)RGNN_WAVE_SMS;
-        if (p.num_incoming != nullptr) seg_reduce_heavy_part_kernel<1, MSG_LINEAR, false, true, false><<<dim3(ix, g128.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        else seg_reduce_heavy_part_kernel<1, MSG_LINEAR, false, false, false><<<dim3(ix, g128.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        seg_reduce_heavy_finish_kernel<1, false><<<dim3(fx, g128.y), WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        count_launch(2);
-      } else if (p.heavy_threshold > 0 && p.heavy_known != 0) {   // heavy targets without scratch: one CTA per target
-        const unsigned hx = p.heavy_known > 0 ? (unsigned)(p.heavy_known < 4 * RGNN_WAVE_SMS ? p.heavy_known : 4 * RGNN_WAVE_SMS) : (unsigned)RGNN_WAVE_SMS;
-        const dim3 hgrid(hx, (p.D + 127) / 128);
-        if (p.num_incoming != nullptr) seg_reduce_heavy_kernel<1, MSG_LINEAR, false, true, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        else seg_reduce_heavy_kernel<1, MSG_LINEAR, false, false, false><<<hgrid, WARPS_PER_BLOCK * 32, 0, stream>>>(p);
-        count_launch();
-      }
-    } else if (seg_cols() == 256 && p.D > 128) launch_seg_nv<2>(p, dim3(gx, (p.D + 255) / 256), stream);
+    const bool use_half = p.msg_mode == MSG_LINEAR && p.agg != RGNN_AGG_MAX && p.act_msg == RGNN_ACT_LINEAR && p.D >= 64 &&
+                          warps128 < (long)RGNN_WAVE_SMS * 40;
+    if (use_half && p.num_incoming != nullptr) launch_seg_half<true>(p, gx, stream);
+    else if (use_half) launch_seg_half<false>(p, gx, stream);
     else launch_seg_nv<1>(p, dim3(gx, (p.D + 127) / 128), stream);
   }
   RGNN_CHECK_CUDA(cudaGetLastError());
@@ -1059,9 +871,8 @@ int launch_seg_rgat(const RgatParams& p, cudaStream_t stream) {
   // one warp per 128-column slice of a target row (heads are independent; more resident warps win here)
   const dim3 grid((p.V + WARPS_PER_BLOCK - 1) / WARPS_PER_BLOCK, (p.D + 127) / 128);
   const int lph = (p.D / p.K) / 4;
-  static const int rgat_half_env = getenv("RGNN_RGAT_HALF") ? atoi(getenv("RGNN_RGAT_HALF")) : -1;   // 0 / 1 force, default: small batches
-  const bool half_ok = p.s_src == nullptr && lph <= 16;
-  if (half_ok && (rgat_half_env == 1 || (rgat_half_env != 0 && (long)p.V * ((p.D + 127) / 128) < (long)RGNN_WAVE_SMS * 40))) {
+  // small batches: twice as many warps, two edges per load instruction (seg_rgat_half_kernel)
+  if (p.s_src == nullptr && lph <= 16 && (long)p.V * ((p.D + 127) / 128) < (long)RGNN_WAVE_SMS * 40) {
     const dim3 hgrid(grid.x, (p.D + 63) / 64);
     RGNN_CHECK_CUDA(launch_pdl(seg_rgat_half_kernel, hgrid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));
   } else if (p.s_src == nullptr) RGNN_CHECK_CUDA(launch_pdl(seg_rgat_kernel<1, true>, grid, dim3(WARPS_PER_BLOCK * 32), 0, stream, p));
@@ -1119,25 +930,6 @@ int launch_act_backward(const float* grad_out, const float* out, const float* pr
   const long n = (long)V * (D / 4);
   if (n == 0) return RGNN_OK;
   act_backward_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(grad_out, out, pre, V, D / 4, act, agg, seg_off, d_agg);
-  RGNN_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  return RGNN_OK;
-}
-
-size_t grad_weight_scratch_floats(int V, int L, int d_in, int d_out) {
-  return (size_t)grad_weight_splits(V, L, d_in, d_out) * L * d_in * d_out;
-}
-
-int launch_grad_weights(const float* h, const float* d_t, int V, int L, int d_in, int d_out, const GradWTable& out,
-                        float* scratch, cudaStream_t stream) {
-  RGNN_REQUIRE((d_in % 4) == 0 && (d_out % 4) == 0, "grad weights: dims must be multiples of 4");
-  const int splits = grad_weight_splits(V, L, d_in, d_out);
-  const dim3 grid((d_out + GW_TILE - 1) / GW_TILE, (d_in + GW_TILE - 1) / GW_TILE, L * splits);
-  grad_weight_partial_kernel<<<grid, 256, 0, stream>>>(h, d_t, V, L, d_in, d_out, splits, scratch);
-  RGNN_CHECK_CUDA(cudaGetLastError());
-  count_launch();
-  const long n = (long)L * d_in * d_out / 4;
-  grad_weight_reduce_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(scratch, L, d_in, d_out, splits, out);
   RGNN_CHECK_CUDA(cudaGetLastError());
   count_launch();
   return RGNN_OK;
