@@ -140,7 +140,15 @@ RGNN_API int rgnn_set_weight_cache(int enable);
 RGNN_API int rgnn_weight_cache_clear(void);
 
 /* Upper bound of the scratch a forward of `layer_kind` needs.  mlp_layers = number of kernels
- * in the widest edge/aggregation MLP (0 if none). */
+ * in the widest edge/aggregation MLP (0 if none).  The bound assumes every MLP layer is at most max(2 * d_in, d_out)
+ * wide (true of the reference's MLPs, whose hidden layers are d_out wide); rgnn_edge_mlp_forward and rgnn_rgin_forward
+ * refuse a wider layer with RGNN_E_UNSUPPORTED before enqueueing anything.
+ *
+ * Workspace contract of every call that takes one: the workspace needs 16-byte alignment only (carve-outs are aligned
+ * relative to its start), its contents on entry are never read, and the call writes nothing past workspace_bytes.  A call
+ * that returns RGNN_E_WORKSPACE (a NULL workspace counts as 0 bytes) has written no output and nothing outside the
+ * workspace; it may already have enqueued kernels that write inside the first workspace_bytes of it (the Edge-MLP, RGIN and
+ * backward paths carve their scratch as they go), so the workspace's contents are undefined afterwards. */
 RGNN_API size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, int32_t d_in, int32_t d_out,
                             int32_t mlp_layers);
 
@@ -170,7 +178,9 @@ RGNN_API int rgnn_rgcn_backward(const rgnn_plan_t* plan, const float* node_embed
 /* graph_num_layers x sparse_rgcn_layer in one call -- the GNN loop of
  * Sparse_Graph_Model.__build_graph_propagation_model (models/sparse_graph_model.py:176-191) without the scaffold's
  * dropout / residual / inter-layer Dense.  edge_weights: host array of num_layers * L pointers (layer-major),
- * every kernel [d, d]; the layers share activation / aggregation / normalisation like RGCN_Model does. */
+ * every kernel [d, d]; the layers share activation / aggregation / normalisation like RGCN_Model does.
+ * Workspace: rgnn_workspace_bytes(plan, RGNN_LAYER_RGCN, d, d, 0) + 2 * (V * d * 4 + 256) bytes (two inter-layer buffers of
+ * [V, d] floats, each rounded up to 256 bytes, then one layer's scratch); less returns RGNN_E_WORKSPACE. */
 RGNN_API int rgnn_rgcn_stack_forward(const rgnn_plan_t* plan, const float* node_embeddings, int32_t d, int32_t num_layers,
                             const float* const* edge_weights, const float* num_incoming,
                             int activation, int aggregation, int normalize_by_num_incoming,
@@ -205,7 +215,8 @@ RGNN_API int rgnn_film_forward(const rgnn_plan_t* plan, const float* node_embedd
 /* ---- gnns/gnn_edge_mlp.py:7-122  sparse_gnn_edge_mlp_layer ---------------------------------
  * mlp_kernels: host array of L * (num_edge_hidden_layers + 1) device pointers, type-major;
  * layer j of every type has shape [mlp_dims[j], mlp_dims[j+1]]; mlp_dims host [layers + 1],
- * mlp_dims[0] = d_in * (1 + use_target_state_as_input), mlp_dims[last] = d_out.
+ * mlp_dims[0] = d_in * (1 + use_target_state_as_input), mlp_dims[last] = d_out, every mlp_dims[j >= 1] at most
+ * max(2 * d_in, d_out) (RGNN_E_UNSUPPORTED otherwise; the same limit holds for both MLPs of rgnn_rgin_forward).
  * Hidden activation is ELU regardless of `activation` (gnn_edge_mlp.py:76). */
 RGNN_API int rgnn_edge_mlp_forward(const rgnn_plan_t* plan, const float* node_embeddings, int32_t d_in, int32_t d_out,
                           const float* const* mlp_kernels, const int32_t* mlp_dims, int num_edge_hidden_layers,

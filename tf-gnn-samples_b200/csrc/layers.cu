@@ -69,6 +69,18 @@ int check_agg(int agg, const char* who) {
   RGNN_REQUIRE(agg >= RGNN_AGG_SUM && agg <= RGNN_AGG_SQRT_N, "%s: Unknown aggregation function code %d", who, agg);
   return RGNN_OK;
 }
+// rgnn_workspace_bytes sizes every scratch row of an MLP layer by max(2 d_in, d_out): a wider MLP layer is refused up
+// front, before anything is enqueued, instead of failing for lack of workspace halfway through the call.
+int check_mlp_widths(const int32_t* dims, int nl, int d_in, int d_out, const char* what, const char* who) {
+  const int limit = (2 * d_in > d_out) ? 2 * d_in : d_out;
+  for (int j = 1; j <= nl; ++j) {
+    if (dims[j] > limit) {
+      set_error("%s: %s layer %d has width %d, above this build's limit max(2 * d_in, d_out) = %d", who, what, j - 1, dims[j], limit);
+      return RGNN_E_UNSUPPORTED;
+    }
+  }
+  return RGNN_OK;
+}
 int check_ws(const Arena& a, const char* who) {
   if (a.overflow) {
     set_error("%s: workspace too small (%zu bytes given, %zu needed)", who, a.cap, a.used);
@@ -459,7 +471,11 @@ extern "C" int rgnn_rgcn_stack_forward(const rgnn_plan_t* plan, const float* h, 
   RGNN_REQUIRE(num_layers == 1 || plan->Vt == plan->V,
                "rgcn_stack: a plan restricted to %d of %d target rows supports num_layers == 1 only (halo rows are not updated)", plan->Vt, plan->V);
   const size_t row_bytes = align_up((size_t)plan->V * d * sizeof(float), 256);
-  RGNN_REQUIRE(workspace != nullptr && workspace_bytes > 2 * row_bytes, "rgcn_stack: workspace too small");
+  if (workspace == nullptr || workspace_bytes <= 2 * row_bytes) {
+    set_error("rgcn_stack: workspace too small (%zu bytes given, more than %zu needed for the two inter-layer buffers)",
+              workspace == nullptr ? (size_t)0 : workspace_bytes, 2 * row_bytes);
+    return RGNN_E_WORKSPACE;
+  }
   char* base = static_cast<char*>(workspace);
   float* buf[2] = {reinterpret_cast<float*>(base), reinterpret_cast<float*>(base + row_bytes)};
   void* inner = base + 2 * row_bytes;
@@ -712,7 +728,6 @@ extern "C" int rgnn_edge_mlp_forward(const rgnn_plan_t* plan, const float* h, in
                                      size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RGNN_PROPAGATE(check_common(plan, h, d_in, d_out, out, num_timesteps, "gnn_edge_mlp"));
-  RGNN_PROPAGATE(plan_wait_sources(plan, stream));
   RGNN_PROPAGATE(check_act(activation, "gnn_edge_mlp"));
   RGNN_PROPAGATE(check_agg(aggregation, "gnn_edge_mlp"));
   RGNN_REQUIRE(mlp_kernels && mlp_dims && ln_gamma && ln_beta, "gnn_edge_mlp: NULL weight pointer");
@@ -720,6 +735,8 @@ extern "C" int rgnn_edge_mlp_forward(const rgnn_plan_t* plan, const float* h, in
   RGNN_REQUIRE(!normalize || num_incoming != nullptr, "gnn_edge_mlp: normalize_by_num_incoming needs type_to_num_incoming_edges");
   const int nl = num_edge_hidden_layers + 1;
   RGNN_REQUIRE(nl <= RGNN_MAX_MLP_LAYERS && mlp_dims[nl] == d_out, "gnn_edge_mlp: MLP output dim %d != state_dim %d", mlp_dims[nl <= RGNN_MAX_MLP_LAYERS ? nl : 0], d_out);
+  RGNN_PROPAGATE(check_mlp_widths(mlp_dims, nl, d_in, d_out, "edge MLP", "gnn_edge_mlp"));
+  RGNN_PROPAGATE(plan_wait_sources(plan, stream));
   const int V = plan->V, D = d_out;
   Arena ar(workspace, workspace_bytes);
   float* buf[2] = {nullptr, nullptr};
@@ -758,7 +775,6 @@ extern "C" int rgnn_rgin_forward(const rgnn_plan_t* plan, const float* h, int32_
                                  void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RGNN_PROPAGATE(check_common(plan, h, d_in, d_out, out, num_timesteps, "rgin"));
-  RGNN_PROPAGATE(plan_wait_sources(plan, stream));
   RGNN_PROPAGATE(check_act(activation, "rgin"));
   RGNN_PROPAGATE(check_agg(aggregation, "rgin"));
   RGNN_REQUIRE(ln_gamma && ln_beta, "rgin: NULL layer-norm parameters");
@@ -766,7 +782,11 @@ extern "C" int rgnn_rgin_forward(const rgnn_plan_t* plan, const float* h, int32_
   const int nl_aggr = num_aggr_mlp_hidden_layers < 0 ? 0 : num_aggr_mlp_hidden_layers + 1;
   RGNN_REQUIRE(nl_edge == 0 || (edge_mlp_kernels && edge_mlp_dims), "rgin: NULL edge MLP table");
   RGNN_REQUIRE(nl_aggr == 0 || (aggr_kernels && aggr_dims), "rgin: NULL aggregation MLP table");
+  RGNN_REQUIRE(nl_edge <= RGNN_MAX_MLP_LAYERS, "rgin: edge MLP too deep");
   RGNN_REQUIRE(nl_aggr <= RGNN_MAX_MLP_LAYERS, "rgin: aggregation MLP too deep");
+  if (nl_edge > 0) RGNN_PROPAGATE(check_mlp_widths(edge_mlp_dims, nl_edge, d_in, d_out, "edge MLP", "rgin"));
+  if (nl_aggr > 0) RGNN_PROPAGATE(check_mlp_widths(aggr_dims, nl_aggr, d_in, d_out, "aggregation MLP", "rgin"));
+  RGNN_PROPAGATE(plan_wait_sources(plan, stream));
   const int V = plan->V, D = d_out;
   Arena ar(workspace, workspace_bytes);
   float* buf[2] = {nullptr, nullptr};
@@ -912,16 +932,21 @@ extern "C" int rgnn_dense_backward(const float* a, int32_t m, int32_t k, const f
                                    float* grad_a, float* grad_b, void* workspace, size_t workspace_bytes, void* stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   RGNN_REQUIRE((grad_c != nullptr || m == 0) && m >= 0 && k > 0 && n > 0 && (k % 4) == 0 && (n % 4) == 0, "dense_backward: bad arguments (m=%d k=%d n=%d)", m, k, n);
-  Arena ar(workspace, workspace_bytes);
-  if (grad_a != nullptr && m > 0) {   // dA = dC . B^T
-    RGNN_REQUIRE(b != nullptr, "dense_backward: grad_a needs b");
-    GemmParams g;
-    g.A1 = grad_c; g.lda1 = n; g.K1 = n; g.M = m; g.N = k; g.C = grad_a; g.ldc = k; g.ldb1 = n;
-    g.batch_mode = BATCH_K_BLOCKS_T; g.batch = 1; g.k_block = n; g.bptr[0] = b; g.bptr2[0] = nullptr;
-    RGNN_PROPAGATE(run_gemm(g, ar, stream));
+  RGNN_REQUIRE(grad_a == nullptr || m == 0 || b != nullptr, "dense_backward: grad_a needs b");
+  RGNN_REQUIRE(grad_b == nullptr || a != nullptr || m == 0, "dense_backward: grad_b needs a");
+  GemmParams g;
+  g.A1 = grad_c; g.lda1 = n; g.K1 = n; g.M = m; g.N = k; g.C = grad_a; g.ldc = k; g.ldb1 = n;
+  g.batch_mode = BATCH_K_BLOCKS_T; g.batch = 1; g.k_block = n; g.bptr[0] = b; g.bptr2[0] = nullptr;
+  {   // size both contractions before launching either: a refused call must not have written grad_a already
+    Arena probe(workspace, workspace_bytes);
+    if (grad_a != nullptr && m > 0) { probe.floats(gemm_tc_pack_bytes(g) / sizeof(float)); if (!probe.overflow) probe.used = 0; }
+    if (grad_b != nullptr) probe.floats(gemm_tn_scratch_floats(k, n, m));
+    RGNN_PROPAGATE(check_ws(probe, "dense_backward"));
   }
+  Arena ar(workspace, workspace_bytes);
+  if (grad_a != nullptr && m > 0)     // dA = dC . B^T
+    RGNN_PROPAGATE(run_gemm(g, ar, stream));
   if (grad_b != nullptr) {            // dB = A^T . dC
-    RGNN_REQUIRE(a != nullptr || m == 0, "dense_backward: grad_b needs a");
     GemmTnOut tn;
     tn.block_cols = n; tn.ld = n; tn.ptr[0] = grad_b;
     float* ws = ar.floats(gemm_tn_scratch_floats(k, n, m));
