@@ -350,6 +350,49 @@ RGNN_API int rgnn_peer_open(const void* handle, void** ptr);
 RGNN_API int rgnn_peer_close(void* ptr);
 RGNN_API int rgnn_peer_free(void* ptr);
 
+/* ---- minibatch packing on the device (tasks/ppi_task.py:197-256, tasks/qm9_task.py:200-261) ------------------------
+ * The task batchers pack graphs into one block-diagonal graph on the host.  Here a whole data set stays on the device,
+ * concatenated in data-set order with GRAPH-LOCAL node ids (CSR over its G graphs and N nodes):
+ *   node_offsets     int64 [G + 1], graph g owns the nodes [node_offsets[g], node_offsets[g + 1])
+ *   edge_offsets     host array of L device pointers, int64 [G + 1] each: graph g's edges of type l are rows
+ *                    [edge_offsets[l][g], edge_offsets[l][g + 1]) of adjacency_lists[l] (int32 [E_l, 2], 8-byte aligned,
+ *                    (source, target) local to the graph, in the graph's own order)
+ *   num_incoming     fp32 [L, N] (in-degrees as the batcher feeds them)
+ *   node_tensors     host array of num_node_tensors device pointers, fp32 [N, node_widths[k]] (features, PPI labels; any
+ *                    width >= 1, no row alignment assumed)
+ *   graph_tensors    host array of num_graph_tensors device pointers, fp32 [graph_rows[k], G] (QM9 targets)
+ * A batch is the graphs order[start], ..., order[start + num_batch_graphs - 1] (order: int32 device array holding at least
+ * start + num_batch_graphs entries, e.g. the epoch's permutation).  Outputs, caller-owned device buffers:
+ *   out_node_tensors[k] [V, w_k], out_adjacency_lists[l] [E_l, 2] (node ids shifted by the graph's first node in the
+ *   batch; batch-graph order, then the graph's own order), out_num_incoming [L, V], out_graph_nodes_list int32 [V] (batch
+ *   index of every node's graph; may be NULL), out_graph_tensors[k] [graph_rows[k], num_batch_graphs].
+ * The values are copies: the result is bit-identical to the host batcher's.  batch_nodes (V) and batch_edges (host [L],
+ * E_l) are the caller's totals, known from host-side per-graph counts; the batch's offsets are computed on the device
+ * (exclusive scans in the workspace).  Nothing is written past the caller's totals.  If a device total differs from the
+ * caller's, or an order entry lies outside [0, G), the pack still completes without a fault, and `status` (int32 device
+ * word, may be NULL) receives RGNN_PACK_* bits -- 0 when the batch is consistent; it is written on every call.
+ * No allocation, no atomics, no synchronisation: capturable into a CUDA graph (a replay reads `order` as it is then).
+ * Workspace: rgnn_pack_workspace_bytes(num_batch_graphs, L), 16-byte aligned (the contract stated above
+ * rgnn_workspace_bytes).  Invalid arguments (negative counts, L outside [1, RGNN_MAX_EDGE_TYPES], more than
+ * RGNN_PACK_MAX_TENSORS tensors of a kind, NULL required pointers) return RGNN_E_INVALID and a short workspace
+ * RGNN_E_WORKSPACE, both before anything is enqueued.  The lists are ready for rgnn_plan_create_ex(...,
+ * RGNN_PLAN_DEFERRED_CHECK) with V = batch_nodes; when the set's local ids were checked against their graphs' sizes once,
+ * no per-batch check is needed. */
+#define RGNN_PACK_MAX_TENSORS 8
+#define RGNN_PACK_NODES_MISMATCH 1   /* the batch's node count differs from batch_nodes */
+#define RGNN_PACK_EDGES_MISMATCH 2   /* some type's edge count differs from batch_edges[l] */
+#define RGNN_PACK_BAD_ORDER 4        /* an order entry lies outside [0, G) (that graph is skipped) */
+RGNN_API size_t rgnn_pack_workspace_bytes(int32_t num_batch_graphs, int32_t num_edge_types);
+RGNN_API int rgnn_pack_minibatch(int64_t num_graphs, int64_t num_nodes, int32_t num_edge_types,
+                        const int64_t* node_offsets, const int64_t* const* edge_offsets,
+                        const int32_t* const* adjacency_lists, const float* num_incoming,
+                        int32_t num_node_tensors, const float* const* node_tensors, const int32_t* node_widths,
+                        int32_t num_graph_tensors, const float* const* graph_tensors, const int32_t* graph_rows,
+                        const int32_t* order, int64_t start, int32_t num_batch_graphs, int32_t batch_nodes,
+                        const int64_t* batch_edges, float* const* out_node_tensors, int32_t* const* out_adjacency_lists,
+                        float* out_num_incoming, int32_t* out_graph_nodes_list, float* const* out_graph_tensors,
+                        int32_t* status, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- building blocks exported for tests / other hosts ---------------------------------------
  * utils/utils.py:23-33: aggregate `data` [M, d] (rows in the ORIGINAL type-major message order)
  * to [V, d] with the plan's segments -- the tf.unsorted_segment_<agg> call of rgcn.py:110. */

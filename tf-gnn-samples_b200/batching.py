@@ -5,7 +5,8 @@ tasks/varmisuse_task.py:451-538): graphs are packed into one block-diagonal grap
 node ids, per-type adjacency lists are concatenated, in-degrees are concatenated along axis 1.
 The reference's datasets are not shipped (data/ppi, data/varmisuse) or not available on the GPU
 box (data/qm9), so the generators below produce seeded, shape-matched synthetic graphs
-(SURVEY.md 8d / Appendix B).  Everything here is numpy on the host, like the reference.
+(SURVEY.md 8d / Appendix B).  Everything here is numpy on the host, like the reference, except DeviceGraphSet at the end:
+the same batches packed on the GPU from a data set uploaded once (rgnn_pack_minibatch).
 """
 from typing import Dict, Iterator, List, NamedTuple, Optional, Sequence, Tuple
 
@@ -271,19 +272,30 @@ def pack_batch(graphs: Sequence[GraphSample], max_nodes_per_batch: Optional[int]
                  graph_node_offsets=np.asarray(offsets, dtype=np.int64))
 
 
-def minibatches(graphs: Sequence[GraphSample], max_nodes_per_batch: int) -> Iterator[Tuple[Batch, int]]:
-    """One epoch of minibatches, the outer loop of tasks/ppi_task.py:211-256 (same in qm9_task.py:212-261): pack graphs in
-    order until the next one would reach the node budget, emit, continue with that graph.  Yields (batch, index of its first
-    graph).  A graph with >= max_nodes_per_batch nodes can never be packed -- the reference then spins on an empty batch
-    (np.concatenate of an empty list raises); here it is a ValueError up front."""
-    start = 0
-    while start < len(graphs):
-        n = graphs[start].node_features.shape[0]
+def batch_bounds(num_nodes: Sequence[int], max_nodes_per_batch: int) -> Iterator[Tuple[int, int]]:
+    """The minibatch boundaries of tasks/ppi_task.py:211-256 (same in qm9_task.py:212-261) from the graphs' node counts alone:
+    add graphs in order while node_offset + |graph| < max_nodes_per_batch, emit, continue with the graph that did not fit.
+    Yields (index of the first graph, number of graphs).  A graph with >= max_nodes_per_batch nodes can never be packed --
+    the reference then spins on an empty batch (np.concatenate of an empty list raises); here it is a ValueError when the
+    loop reaches it."""
+    start, count = 0, len(num_nodes)
+    while start < count:
+        n = int(num_nodes[start])
         if not (n < max_nodes_per_batch):
             raise ValueError("graph %d has %d nodes: does not fit max_nodes_per_batch=%d" % (start, n, max_nodes_per_batch))
-        batch = pack_batch(graphs[start:], max_nodes_per_batch)
-        yield batch, start
-        start += batch.num_graphs
+        end, offset = start, 0
+        while end < count and offset + int(num_nodes[end]) < max_nodes_per_batch:
+            offset += int(num_nodes[end])
+            end += 1
+        yield start, end - start
+        start = end
+
+
+def minibatches(graphs: Sequence[GraphSample], max_nodes_per_batch: int) -> Iterator[Tuple[Batch, int]]:
+    """One epoch of minibatches, the outer loop of tasks/ppi_task.py:211-256 (same in qm9_task.py:212-261), with the
+    boundaries of ``batch_bounds``.  Yields (batch, index of its first graph)."""
+    for start, count in batch_bounds([g.node_features.shape[0] for g in graphs], max_nodes_per_batch):
+        yield pack_batch(graphs[start:start + count]), start
 
 
 def ppi_like_batch(num_graphs: int = 1, num_nodes: int = 2245, num_links: int = 59000, seed: int = 0,
@@ -310,3 +322,207 @@ def varmisuse_like_batch(num_nodes: int = 50000, num_edges: int = 1000000, packe
     n, e = num_nodes // packed_graphs, num_edges // packed_graphs
     return pack_batch([make_typed_random_graph(n, e, VARMISUSE_TYPE_FRACTIONS, feature_dim, seed + i)
                        for i in range(packed_graphs)])
+
+
+# ---- minibatches packed on the GPU from a device-resident graph set (rgnn_pack_minibatch in include/rgnn.h) ----
+class DeviceBatch:
+    """One minibatch packed on the device: the tensors of a reference feed (tasks/sparse_graph_task.py:139-149) plus the
+    counters ``training.run_epoch`` reads.  ``args()`` returns what ``training.device_args`` returns for the same batch, so
+    ``run_epoch(..., batches=graph_set.minibatches(budget, order), to_device=lambda b: b.args())`` trains on it unchanged."""
+
+    def __init__(self, graph_set, num_graphs, num_nodes, num_edges, node_tensors, adjacency_lists, num_incoming,
+                 graph_nodes_list, graph_tensors, status):
+        self.graph_set = graph_set
+        self.num_graphs, self.num_nodes, self.num_edges = num_graphs, num_nodes, num_edges
+        self.node_features = node_tensors[0]                # float32 [V, D0]
+        self.node_tensors = node_tensors                    # [0] = features, then the set's extra per-node tensors
+        self.adjacency_lists = adjacency_lists              # L x int32 [E_l, 2]; a type without edges is [0, 2]
+        self.type_to_num_incoming_edges = num_incoming      # float32 [L, V]
+        self.graph_nodes_list = graph_nodes_list            # int32 [V]
+        self.graph_tensors = graph_tensors                  # float32 [T_k, num_graphs] each
+        self.status = status                                # int32 [1]: RGNN_PACK_* bits, 0 = consistent
+
+    @property
+    def batch(self) -> "DeviceBatch":
+        """The counters live on the batch itself (run_epoch reads ``tb.batch.num_graphs`` of a TaskBatch)."""
+        return self
+
+    @property
+    def targets(self):
+        """PPI: the node labels [V, num_labels]; QM9: the target values [len(task_ids), num_graphs]."""
+        kind = self.graph_set.targets_kind
+        if kind == "graph":
+            return self.graph_tensors[0]
+        return self.node_tensors[1] if kind == "node" else None
+
+    def args(self) -> Tuple:
+        """(features, plan, num_incoming, targets[, graph_nodes_list, num_graphs]), like training.device_args.  The plan is
+        built without validation (no synchronisation): the graph set checked every node id when it was uploaded."""
+        from .engine import GraphPlan
+        plan = GraphPlan(self.adjacency_lists, self.num_nodes, device=self.node_features.device, validate=False)
+        args = (self.node_features, plan, self.type_to_num_incoming_edges, self.targets)
+        if self.graph_set.targets_kind == "graph":
+            args += (self.graph_nodes_list, self.num_graphs)
+        return args
+
+    def check(self):
+        """Synchronise and raise RgnnError if the device-computed totals disagreed with the host's or ``order`` held an id
+        outside the set (the status word of rgnn_pack_minibatch)."""
+        from .engine import RGNN_E_INVALID, RgnnError
+        st = int(self.status.item())
+        if st != 0:
+            raise RgnnError(RGNN_E_INVALID, "pack_minibatch: status %d (1 = node total, 2 = edge total differs from the "
+                                            "host's; 4 = order entry outside the graph set)" % st)
+
+
+class DeviceGraphSet:
+    """A whole data set uploaded once, packed into minibatches on the GPU (one rgnn_pack_minibatch per batch: no per-batch
+    host-to-device copy, no Python loop over graphs, no synchronisation).  Feed for feed the batches equal ``minibatches``
+    over ``[graphs[i] for i in order]``, bit for bit.
+
+    Layout (CSR over graphs, data-set order, graph-local node ids): node offsets int64 [G + 1]; per edge type edge offsets
+    int64 [G + 1] and edges int32 [E_l, 2]; in-degrees float32 [L, N]; per-node tensors float32 [N, w] (``node_tensors[0]``
+    is the node features; ``node_tensors`` adds more, each a per-graph sequence of [V_g, w] arrays, e.g. PPI labels);
+    per-graph tensors float32 [T, G] (``graph_tensors``: one [T, G] array or a sequence of them, e.g. QM9 targets).
+    ``targets`` of a batch: the first per-graph tensor if there is one (and ``args()`` then carries graph_nodes_list and
+    num_graphs like a QM9 feed), else the first extra per-node tensor (a PPI feed).
+
+    Every node id is checked against its graph's size once, here on the host (RgnnError on a violation), so the per-batch
+    GraphPlan needs no validation."""
+
+    def __init__(self, graphs: Sequence[GraphSample], device=None, node_tensors: Sequence[Sequence[np.ndarray]] = (),
+                 graph_tensors=None):
+        import torch
+        from .engine import RGNN_E_INVALID, RgnnError
+        graphs = list(graphs)
+        if not graphs:
+            raise ValueError("DeviceGraphSet needs at least one graph")
+        if device is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        self.device = torch.device(device)
+        G, L = len(graphs), len(graphs[0].adjacency_lists)
+        if any(len(g.adjacency_lists) != L for g in graphs):
+            raise ValueError("every graph needs the same number of edge types (%d)" % L)
+        sizes = np.array([g.node_features.shape[0] for g in graphs], dtype=np.int64)
+        node_off = np.zeros(G + 1, dtype=np.int64)
+        np.cumsum(sizes, out=node_off[1:])
+        edge_counts = np.zeros((L, G), dtype=np.int64)
+        edge_off, edges = [], []
+        for l in range(L):
+            lists = [np.asarray(g.adjacency_lists[l]).reshape(-1, 2) for g in graphs]
+            edge_counts[l] = [a.shape[0] for a in lists]
+            off = np.zeros(G + 1, dtype=np.int64)
+            np.cumsum(edge_counts[l], out=off[1:])
+            cat = np.concatenate(lists).astype(np.int64) if off[-1] > 0 else np.zeros((0, 2), dtype=np.int64)
+            bad = ((cat < 0) | (cat >= np.repeat(sizes, edge_counts[l])[:, None])).any(axis=1)
+            if bad.any():
+                e = int(np.argmax(bad))
+                g = int(np.searchsorted(off, e, side="right") - 1)
+                raise RgnnError(RGNN_E_INVALID, "graph %d, edge type %d: edge %s holds a node index outside [0, %d)"
+                                % (g, l, tuple(int(x) for x in cat[e]), sizes[g]))
+            edge_off.append(off)
+            edges.append(cat.astype(np.int32))
+        indeg = [np.asarray(g.type_to_node_to_num_incoming_edges) for g in graphs]
+        if any(d.shape != (L, n) for d, n in zip(indeg, sizes)):
+            raise ValueError("in-degrees must be [L, V_g] for every graph")
+        indeg = np.concatenate(indeg, axis=1)
+        per_node = [[g.node_features for g in graphs]] + [list(t) for t in node_tensors]
+        node_arrays = []
+        for k, parts in enumerate(per_node):
+            parts = [np.asarray(p, dtype=np.float32) for p in parts]
+            if len(parts) != G or any(p.ndim != 2 or p.shape != (n, parts[0].shape[1]) for p, n in zip(parts, sizes)):
+                raise ValueError("per-node tensor %d must hold one [V_g, w] array per graph, w the same for all" % k)
+            node_arrays.append(np.concatenate(parts, axis=0))
+        if graph_tensors is None:
+            graph_tensors = []
+        elif isinstance(graph_tensors, np.ndarray):
+            graph_tensors = [graph_tensors]
+        graph_arrays = [np.asarray(t, dtype=np.float32).reshape(-1, G) for t in graph_tensors]
+        if len(node_arrays) > 8 or len(graph_arrays) > 8:       # RGNN_PACK_MAX_TENSORS
+            raise ValueError("at most 8 per-node tensors (features included) and 8 per-graph tensors")
+
+        def up(a):
+            return torch.from_numpy(np.ascontiguousarray(a)).to(self.device)
+        self.num_graphs, self.num_nodes, self.num_edge_types = G, int(node_off[-1]), L
+        self.graph_sizes, self.edge_counts = sizes, edge_counts          # host-side counts: batch boundaries and totals
+        self.node_offsets = up(node_off)
+        self.edge_offsets = [up(o) for o in edge_off]
+        self.adjacency_lists = [up(e) for e in edges]
+        self.num_incoming = up(indeg.astype(np.float32))
+        self.node_tensors = [up(a) for a in node_arrays]
+        self.graph_tensors = [up(a) for a in graph_arrays]
+        self.targets_kind = "graph" if graph_arrays else ("node" if len(node_arrays) > 1 else None)
+
+    @classmethod
+    def from_qm9_records(cls, records: Sequence[Dict], add_self_loop_edges: bool = True, tie_fwd_bkwd_edges: bool = True,
+                         task_ids: Sequence[int] = (0,), device=None) -> "DeviceGraphSet":
+        """QM9 records (load_qm9_jsonl) converted once, as qm9_batch converts them per batch; targets [len(task_ids), G]."""
+        L = qm9_num_edge_types(records, add_self_loop_edges, tie_fwd_bkwd_edges)
+        samples = [qm9_graph_to_sample(r, L, add_self_loop_edges, tie_fwd_bkwd_edges) for r in records]
+        targets = np.array([[r["targets"][t][0] for r in records] for t in task_ids], dtype=np.float32).reshape(-1, len(records))
+        return cls(samples, device, graph_tensors=targets)
+
+    @classmethod
+    def from_ppi_fold(cls, graphs: Sequence[GraphSample], labels: Sequence[np.ndarray], device=None) -> "DeviceGraphSet":
+        """A PPI fold as load_ppi_fold returns it; the per-node labels [V_g, num_labels] become the batches' targets."""
+        return cls(graphs, device, node_tensors=(labels,))
+
+    def _host_order(self, order) -> np.ndarray:
+        if order is None:
+            return np.arange(self.num_graphs, dtype=np.int32)
+        order = np.asarray(order).reshape(-1)
+        if order.size and (order.min() < 0 or order.max() >= self.num_graphs):
+            raise ValueError("order holds a graph index outside [0, %d)" % self.num_graphs)
+        return order.astype(np.int32)
+
+    def upload_order(self, order=None):
+        """(host int32 order, device int32 copy): the epoch's graph order, checked on the host, copied once from pinned
+        memory without synchronising.  None = data-set order."""
+        import torch
+        order = self._host_order(order)
+        return order, torch.from_numpy(order).pin_memory().to(self.device, non_blocking=True)
+
+    def pack(self, order: np.ndarray, order_dev, start: int, count: int) -> DeviceBatch:
+        """Pack the graphs order[start : start + count] on the current stream.  ``order`` is the host copy of ``order_dev``
+        (the totals come from it); the kernel reads ``order_dev``, so a CUDA graph that captured this call packs whatever
+        order_dev holds when it is replayed."""
+        import ctypes
+        import torch
+        from .engine import check, current_stream_ptr, load_library, ptr_table, workspace
+        lib = load_library()
+        L, dev = self.num_edge_types, self.device
+        sel = order[start:start + count]
+        V = int(self.graph_sizes[sel].sum())
+        E = [int(x) for x in self.edge_counts[:, sel].sum(axis=1)]
+        nodes = [torch.empty((V, t.shape[1]), dtype=torch.float32, device=dev) for t in self.node_tensors]
+        adj = [torch.empty((e, 2), dtype=torch.int32, device=dev) for e in E]
+        indeg = torch.empty((L, V), dtype=torch.float32, device=dev)
+        gnl = torch.empty(V, dtype=torch.int32, device=dev)
+        per_graph = [torch.empty((t.shape[0], count), dtype=torch.float32, device=dev) for t in self.graph_tensors]
+        status = torch.empty(1, dtype=torch.int32, device=dev)
+        ws_bytes = int(lib.rgnn_pack_workspace_bytes(count, L))
+        ws = workspace(dev, ws_bytes)
+        widths = (ctypes.c_int32 * 8)(*[t.shape[1] for t in self.node_tensors])
+        rows = (ctypes.c_int32 * 8)(*[t.shape[0] for t in self.graph_tensors])
+        with torch.cuda.device(dev):
+            check(lib.rgnn_pack_minibatch(
+                self.num_graphs, self.num_nodes, L, self.node_offsets.data_ptr(),
+                ptr_table(self.edge_offsets, weights=False), ptr_table(self.adjacency_lists, weights=False),
+                self.num_incoming.data_ptr(),
+                len(self.node_tensors), ptr_table(self.node_tensors, weights=False), widths,
+                len(self.graph_tensors), ptr_table(self.graph_tensors, weights=False), rows,
+                order_dev.data_ptr(), int(start), int(count), V, (ctypes.c_int64 * L)(*E),
+                ptr_table(nodes, weights=False), ptr_table(adj, weights=False), indeg.data_ptr(), gnl.data_ptr(),
+                ptr_table(per_graph, weights=False), status.data_ptr(), ws.data_ptr(), ws.numel(),
+                current_stream_ptr(dev)))
+        return DeviceBatch(self, int(count), V, int(sum(E)), nodes, adj, indeg, gnl, per_graph, status)
+
+    def minibatches(self, max_nodes_per_batch: int, order=None) -> Iterator[DeviceBatch]:
+        """One epoch: the batches ``minibatches([graphs[i] for i in order], max_nodes_per_batch)`` yields, packed on the
+        device.  ``order`` is the caller's shuffle (the reference shuffles the training fold every epoch); it is uploaded
+        once.  Every boundary is computed, and a graph that can never fit raises ValueError, before anything is launched."""
+        order_host = self._host_order(order)
+        bounds = list(batch_bounds(self.graph_sizes[order_host], max_nodes_per_batch))
+        order_host, order_dev = self.upload_order(order_host)
+        for start, count in bounds:
+            yield self.pack(order_host, order_dev, start, count)

@@ -90,6 +90,10 @@ SIGNATURES = {
     "rgnn_peer_free": (c_int, [_PTR]),
     "rgnn_rgcn_stack_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, c_int, c_int, c_int,
                                         _PTR, _PTR, c_size_t, _PTR]),
+    "rgnn_pack_workspace_bytes": (c_size_t, [c_int32, c_int32]),
+    "rgnn_pack_minibatch": (c_int, [c_int64, c_int64, c_int32, _PTR, _PTR, _PTR, _PTR, c_int32, _PTR, _PTR, c_int32, _PTR,
+                                    _PTR, _PTR, c_int64, c_int32, c_int32, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR,
+                                    c_size_t, _PTR]),
 }
 OPTIONAL_SYMBOLS = set()
 
