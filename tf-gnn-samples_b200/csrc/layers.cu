@@ -6,6 +6,7 @@
 // is one fused sorted-segment kernel (seg_kernels.cu).  RGAT already works this way in the reference
 // (rgat.py:95-96).  Only an MLP's layers after a per-edge nonlinearity stay per-edge (edge-MLP with
 // >= 1 hidden layer and target input): those run as per-type row-range GEMMs over materialised rows.
+#include <algorithm>
 #include <mutex>
 #include <atomic>
 #include <string.h>
@@ -318,6 +319,11 @@ extern "C" size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, 
       break;
     }
     case RGNN_LAYER_RGDCN: floats = V * L * dm * (size_t)(mlp_layers > 0 ? mlp_layers : 16) + 2 * V * dm; break;   // mlp_layers carries channel_dim
+    case RGNN_LAYER_FILM_BACKWARD: {   // T, dT [V, L, D]; FW, dFW [Vt <= V, L, 2D]; d_a [Vt, D]; the second d_h term [Vt, d_in];
+      const size_t di = (size_t)d_in, dd = (size_t)d_out;   // LN partials; split-K tiles of d_W / d_F
+      floats = 6 * V * L * dd + V * (dd + di) + (size_t)FILM_LN_MAX_BLOCKS * 2 * dd + (RGNN_WAVE_SMS * 16384 + 2 * L * di * dd) + 64 * 1024;
+      break;
+    }
     default: return 0;
   }
   // scratch for the pre-swizzled hi/lo weight images of the largest dense contraction of the layer
@@ -713,6 +719,141 @@ extern "C" int rgnn_film_forward(const rgnn_plan_t* plan, const float* h, int32_
     s.out = dst; s.ld_out = D; s.heavy_scratch = heavy.heavy_scratch;
     RGNN_PROPAGATE(launch_seg_reduce(s, stream));
     cur = dst; din = D;
+  }
+  return RGNN_OK;
+}
+
+// Backward of ONE timestep of sparse_gnn_film_layer: what tf.gradients produces for gnns/gnn_film.py:85-120.  No forward
+// state is kept: the tables are recomputed (film_backward.cu has the math).
+//   T = h . [W_0|..|W_{L-1}] (V rows), FW = h . [F_0|..|F_{L-1}] (Vt rows), a = agg act(gamma * s T + beta) (segment reduce)
+//   d_a = LayerNorm backward / div                          d_ln_gamma, d_ln_beta: per-CTA partials, fixed-order sum
+//   dFW[v,l] = [sum g_e s T[u,l] | sum g_e]  (CSR by target)  dT[u,l] = sum s gamma[v,l] g_e  (reverse index)
+//   d_h = dT . [W_l]^T (V rows) + dFW . [F_l]^T (Vt rows)   two transposed-image GEMMs, added in that order
+//   d_W_l = h^T . dT[:, l, :],  d_F_l = h[:Vt]^T . dFW[:, l, :]   TN GEMMs, split-K, deterministic
+extern "C" int rgnn_film_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d_in, int32_t d_out,
+                                  const float* const* edge_weights, const float* const* film_weights,
+                                  const float* num_incoming, const float* ln_gamma, const float* ln_beta, int activation,
+                                  int aggregation, int normalize, const float* grad_out, float* grad_h,
+                                  float* const* grad_edge_weights, float* const* grad_film_weights, float* grad_ln_gamma,
+                                  float* grad_ln_beta, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  rgnn_plan* plan = const_cast<rgnn_plan*>(plan_c);   // the reverse index is built lazily inside the plan
+  RGNN_REQUIRE(plan != nullptr && h != nullptr && grad_out != nullptr && edge_weights != nullptr && film_weights != nullptr &&
+               ln_gamma != nullptr && ln_beta != nullptr, "film_backward: NULL argument");
+  RGNN_REQUIRE(d_in > 0 && d_out > 0 && (d_in % 4) == 0 && (d_out % 4) == 0,
+               "film_backward: dims must be positive multiples of 4 (d_in=%d, d_out=%d)", d_in, d_out);
+  if (d_out > RGNN_MAX_STATE_DIM) {
+    set_error("film_backward: state dim %d > %d (the layer norm holds a row per warp) is not supported", d_out, RGNN_MAX_STATE_DIM);
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_PROPAGATE(check_act(activation, "film_backward"));
+  RGNN_PROPAGATE(check_agg(aggregation, "film_backward"));
+  if (aggregation == RGNN_AGG_MAX) {
+    set_error("film_backward: the gradient of 'max' aggregation is not implemented in this build");
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_REQUIRE(!normalize || num_incoming != nullptr, "film_backward: normalize_by_num_incoming needs type_to_num_incoming_edges");
+  RGNN_REQUIRE(aligned16(h) && aligned16(grad_out) && aligned16(ln_gamma) && aligned16(ln_beta) && aligned16(grad_h) &&
+               aligned16(grad_ln_gamma) && aligned16(grad_ln_beta), "film_backward: buffers must be 16-byte aligned");
+  RGNN_REQUIRE(grad_h != h, "film_backward: grad_node_embeddings must not alias node_embeddings");
+  const int V = plan->V, Vt = plan->Vt, L = plan->L, D = d_out;
+  for (int l = 0; l < L; ++l) {
+    RGNN_REQUIRE(edge_weights[l] != nullptr && film_weights[l] != nullptr, "film_backward: weight %d is NULL", l);
+    RGNN_REQUIRE(grad_edge_weights == nullptr || (grad_edge_weights[l] != nullptr && aligned16(grad_edge_weights[l])),
+                 "film_backward: grad edge weight %d is NULL / misaligned", l);
+    RGNN_REQUIRE(grad_film_weights == nullptr || (grad_film_weights[l] != nullptr && aligned16(grad_film_weights[l])),
+                 "film_backward: grad film weight %d is NULL / misaligned", l);
+  }
+
+  // every carve-out and the largest weight-image scratch of the four dense contractions, before anything is enqueued
+  Arena ar(workspace, workspace_bytes);
+  float* T = ar.floats((size_t)V * L * D);
+  float* FW = ar.floats((size_t)Vt * L * 2 * D);
+  float* dT = ar.floats((size_t)V * L * D);
+  float* dFW = ar.floats((size_t)Vt * L * 2 * D);
+  float* a = ar.floats((size_t)Vt * D);                       // the aggregate, then d_a in place
+  const bool want_ln = grad_ln_gamma != nullptr || grad_ln_beta != nullptr;
+  float* ln_part = ar.floats((size_t)film_ln_blocks(Vt) * 2 * D + 4);
+  float* gh_tail = grad_h != nullptr ? ar.floats((size_t)Vt * d_in + 4) : nullptr;   // dFW . [F_l]^T
+  float* tn_scratch = nullptr;
+  if (grad_edge_weights != nullptr || grad_film_weights != nullptr) {
+    const size_t a1 = gemm_tn_scratch_floats(d_in, L * D, V), a2 = gemm_tn_scratch_floats(d_in, L * 2 * D, Vt);
+    tn_scratch = ar.floats(a1 > a2 ? a1 : a2);
+  }
+  SegParams heavy;
+  seg_heavy_scratch(heavy, plan, ar, D);
+  GemmParams gT, gF, gH1, gH2;
+  gT.A1 = h; gT.lda1 = d_in; gT.K1 = d_in; gT.M = V; gT.N = D; gT.C = T; gT.ldc = L * D; gT.ldb1 = D;
+  gT.batch_mode = BATCH_SHARED_A; gT.batch = L;
+  gF = gT;
+  gF.M = Vt; gF.N = 2 * D; gF.C = FW; gF.ldc = L * 2 * D; gF.ldb1 = 2 * D;
+  gH1.A1 = dT; gH1.lda1 = L * D; gH1.K1 = L * D; gH1.M = V; gH1.N = d_in; gH1.C = grad_h; gH1.ldc = d_in; gH1.ldb1 = D;
+  gH1.batch_mode = BATCH_K_BLOCKS_T; gH1.batch = L; gH1.k_block = D;
+  gH2 = gH1;
+  gH2.A1 = dFW; gH2.lda1 = L * 2 * D; gH2.K1 = L * 2 * D; gH2.M = Vt; gH2.C = gh_tail; gH2.ldb1 = 2 * D; gH2.k_block = 2 * D;
+  for (int l = 0; l < L; ++l) {
+    gT.bptr[l] = edge_weights[l]; gF.bptr[l] = film_weights[l]; gH1.bptr[l] = edge_weights[l]; gH2.bptr[l] = film_weights[l];
+    gT.bptr2[l] = gF.bptr2[l] = gH1.bptr2[l] = gH2.bptr2[l] = nullptr;
+  }
+  size_t pack = gemm_tc_pack_bytes(gT);
+  if (Vt > 0) pack = std::max(pack, gemm_tc_pack_bytes(gF));
+  if (grad_h != nullptr) pack = std::max(pack, std::max(gemm_tc_pack_bytes(gH1), Vt > 0 ? gemm_tc_pack_bytes(gH2) : (size_t)0));
+  {
+    const size_t mark = ar.used;
+    ar.floats(pack / sizeof(float));
+    RGNN_PROPAGATE(check_ws(ar, "film_backward"));
+    ar.used = mark;
+  }
+  RGNN_PROPAGATE(plan_ensure_reverse(plan, stream));
+  RGNN_PROPAGATE(plan_wait_sources(plan, stream));   // T reads the halo rows
+
+  // forward tables and the aggregate (no layer-norm epilogue)
+  if (Vt > 0) RGNN_PROPAGATE(run_gemm(gF, ar, stream));
+  RGNN_PROPAGATE(run_gemm(gT, ar, stream));
+  {
+    SegParams s;
+    seg_from_plan(s, plan);
+    s.D = D; s.table = T; s.stride_idx = (long)L * D; s.stride_type = D;
+    s.num_incoming = normalize ? num_incoming : nullptr;
+    s.msg_mode = MSG_FILM; s.mod_table = FW; s.mod_stride_node = (long)L * 2 * D; s.mod_stride_type = 2 * D;
+    s.act_msg = activation; s.agg = aggregation;
+    s.out = a; s.ld_out = D; s.heavy_scratch = heavy.heavy_scratch;
+    RGNN_PROPAGATE(launch_seg_reduce(s, stream));
+  }
+  FilmLnBwdParams lp;
+  lp.rows = Vt; lp.D = D; lp.agg = aggregation; lp.seg_off = plan->seg_off; lp.grad_out = grad_out; lp.ln_gamma = ln_gamma;
+  lp.a = a; lp.partial = ln_part;
+  RGNN_PROPAGATE(launch_film_ln_backward(lp, stream));
+  FilmBwdParams ep;
+  ep.V = V; ep.Vt = Vt; ep.L = L; ep.D = D; ep.act = activation;
+  ep.seg_off = plan->seg_off; ep.e_src = plan->e_src; ep.e_type = plan->e_type;
+  ep.heavy_list = plan->heavy_list; ep.heavy_count = plan->err_flag + 1;
+  ep.rev_off = plan->rev_seg_off; ep.rev_tgt = plan->rev_src;
+  ep.rev_heavy_list = plan->rev_heavy_list; ep.rev_heavy_count = plan->err_flag + 2;
+  ep.T = T; ep.FW = FW; ep.d_a = a; ep.num_incoming = normalize ? num_incoming : nullptr; ep.scale_ld = V;
+  ep.dT = dT; ep.dFW = dFW;
+  RGNN_PROPAGATE(launch_film_edge_backward(ep, plan->num_heavy_host, stream));
+
+  // the outputs, each written once
+  if (want_ln) RGNN_PROPAGATE(launch_film_ln_param_reduce(ln_part, Vt, D, grad_ln_gamma, grad_ln_beta, stream));
+  if (grad_edge_weights != nullptr) {
+    GemmTnOut tn;
+    tn.block_cols = D; tn.ld = D;
+    for (int l = 0; l < L; ++l) tn.ptr[l] = grad_edge_weights[l];
+    RGNN_PROPAGATE(launch_gemm_tn(h, d_in, dT, L * D, d_in, L * D, V, tn, tn_scratch, stream));
+  }
+  if (grad_film_weights != nullptr) {
+    GemmTnOut tn;
+    tn.block_cols = 2 * D; tn.ld = 2 * D;
+    for (int l = 0; l < L; ++l) tn.ptr[l] = grad_film_weights[l];
+    RGNN_PROPAGATE(launch_gemm_tn(h, d_in, dFW, L * 2 * D, d_in, L * 2 * D, Vt, tn, tn_scratch, stream));
+  }
+  if (grad_h != nullptr) {
+    if (V > 0) RGNN_PROPAGATE(run_gemm(gH1, ar, stream));
+    if (Vt > 0) {
+      RGNN_PROPAGATE(run_gemm(gH2, ar, stream));
+      RGNN_PROPAGATE(launch_add_rows(grad_h, gh_tail, (long)Vt * d_in, stream));
+    }
   }
   return RGNN_OK;
 }

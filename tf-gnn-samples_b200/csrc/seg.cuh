@@ -108,4 +108,43 @@ int launch_layer_norm(const float* x, int rows, int D, const float* gamma, const
 int launch_act_backward(const float* grad_out, const float* out, const float* pre, int V, int D, int act, int agg,
                         const int32_t* seg_off, float* d_agg, cudaStream_t stream);
 
+// ---- rgnn_film_backward (film_backward.cu) ----
+// LayerNorm backward of one FiLM timestep: a [rows, D] (the recomputed aggregate) is overwritten with
+// d_a = rstd (g - mean(g) - x_hat mean(g x_hat)) / div(v), g = grad_out * ln_gamma; per-CTA partial sums of grad_out * x_hat
+// and grad_out go to partial [film_ln_blocks(rows), 2D] and are added in CTA order into d_gamma / d_beta (either may be NULL).
+struct FilmLnBwdParams {
+  int rows = 0, D = 0, agg = RGNN_AGG_SUM;
+  const int32_t* seg_off = nullptr;    // divisor of mean / sqrt_n: all incoming edges of v
+  const float* grad_out = nullptr;
+  const float* ln_gamma = nullptr;
+  float* a = nullptr;
+  float* partial = nullptr;
+};
+constexpr int FILM_LN_MAX_BLOCKS = 2 * RGNN_WAVE_SMS;
+inline int film_ln_blocks(int rows) {
+  const int b = (rows + 7) / 8;
+  return b < FILM_LN_MAX_BLOCKS ? b : FILM_LN_MAX_BLOCKS;
+}
+int launch_film_ln_backward(const FilmLnBwdParams& p, cudaStream_t stream);
+int launch_film_ln_param_reduce(const float* partial, int rows, int D, float* d_gamma, float* d_beta, cudaStream_t stream);
+
+// The two edge kernels: dFW [Vt, L, 2D] over the CSR by target, dT [V, L, D] over the reverse index.
+struct FilmBwdParams {
+  int V = 0, Vt = 0, L = 1, D = 0, act = RGNN_ACT_LINEAR;
+  const int32_t* seg_off = nullptr; const int32_t* e_src = nullptr; const int32_t* e_type = nullptr;
+  const int32_t* heavy_list = nullptr; const int* heavy_count = nullptr;          // targets above RGNN_HEAVY_SEGMENT
+  const int32_t* rev_off = nullptr; const int32_t* rev_tgt = nullptr;             // segment u * L + l, entry = target
+  const int32_t* rev_heavy_list = nullptr; const int* rev_heavy_count = nullptr;
+  const float* T = nullptr;            // [V, L, D]   h . [W_0 | .. | W_{L-1}]
+  const float* FW = nullptr;           // [Vt, L, 2D] h . [F_0 | .. | F_{L-1}]  (gamma | beta)
+  const float* d_a = nullptr;          // [Vt, D]
+  const float* num_incoming = nullptr; // [L, scale_ld] or NULL
+  int scale_ld = 0;
+  float* dT = nullptr;
+  float* dFW = nullptr;
+};
+int launch_film_edge_backward(const FilmBwdParams& p, int heavy_known, cudaStream_t stream);
+// y[0:n] += x[0:n]  (n % 4 == 0)
+int launch_add_rows(float* y, const float* x, long n, cudaStream_t stream);
+
 }  // namespace rgnn
