@@ -24,7 +24,8 @@
  *             rgnn_set_weight_cache(0) call cudaFree: never call them during a capture.
  *   capture   run eagerly once before capturing: every layer with the weight cache on (a cache miss
  *             during capture is an error), and the first backward on a plan (rgnn_rgcn_backward /
- *             rgnn_film_backward / rgnn_edge_aggregate_backward build the plan's reverse index then; inside a capture they
+ *             rgnn_film_backward / rgnn_rgat_backward / rgnn_edge_aggregate_backward build the plan's reverse index then;
+ *             inside a capture they
  *             return RGNN_E_INVALID).  A plan built with RGNN_PLAN_DEFERRED_CHECK inside a capture is
  *             filled only when the graph is replayed: call rgnn_plan_status after a replay.  A graph
  *             captured with the weight cache on reads the cached images: rgnn_weight_cache_clear (and
@@ -84,7 +85,7 @@ enum rgnn_layer_kind {
   RGNN_LAYER_RGCN = 0, RGNN_LAYER_GGNN = 1, RGNN_LAYER_RGAT = 2, RGNN_LAYER_FILM = 3,
   RGNN_LAYER_EDGE_MLP = 4, RGNN_LAYER_RGIN = 5, RGNN_LAYER_RGCN_BACKWARD = 6,
   RGNN_LAYER_RGDCN = 7,  /* rgnn_workspace_bytes: pass channel_dim as mlp_layers */
-  RGNN_LAYER_FILM_BACKWARD = 8
+  RGNN_LAYER_FILM_BACKWARD = 8, RGNN_LAYER_RGAT_BACKWARD = 9
 };
 
 typedef struct rgnn_plan rgnn_plan_t;
@@ -203,6 +204,29 @@ RGNN_API int rgnn_rgat_forward(const rgnn_plan_t* plan, const float* node_embedd
                       const float* const* edge_weights, const float* const* attention,
                       int num_heads, int activation, int num_timesteps,
                       float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of ONE timestep of sparse_rgat_layer (rgat.py:83-139): the gradients TensorFlow autodiff produces.
+ * Gradients are written, not accumulated.  No forward state is needed: the call recomputes h . W_l, the per-head scores
+ * and the softmax from its inputs, and builds no per-edge tensor.
+ *   node_embeddings [V, d_in]: this timestep's INPUT; attention: as rgnn_rgat_forward (16-byte aligned)
+ *   grad_out [num_targets, d_out] (rows [0, num_targets) of the plan, rgnn_plan_set_num_targets)
+ *   grad_node_embeddings [V, d_in] covers EVERY local row (halo rows included: what rgnn_halo_exchange_backward consumes)
+ *   or NULL; grad_edge_weights: host array of L device pointers [d_in, d_out] or NULL; grad_attention: host array of L
+ *   device pointers [2 * d_out] or NULL.
+ * d_out > RGNN_MAX_STATE_DIM and per-head dims d_out / num_heads that are not multiples of 4 return RGNN_E_UNSUPPORTED;
+ * num_heads must divide d_out.  Every argument is checked and the workspace sized before anything is enqueued.  The first
+ * backward on a plan builds its reverse index (as rgnn_rgcn_backward; not inside a capture).  Two identical calls are
+ * bit-identical (no atomics: every output has one writer, every sum a fixed order).
+ * Several timesteps are the caller's loop: run the forward with num_timesteps = 1 per timestep keeping each input, call
+ * this from the last timestep down (grad_out of step t = grad_node_embeddings of step t + 1), and add the shared weights'
+ * gradients of the steps.
+ * Workspace: rgnn_workspace_bytes(plan, RGNN_LAYER_RGAT_BACKWARD, d_in, d_out, 0), a bound for every head count: with
+ * V = num_nodes, L = num_edge_types, D = d_out, (3 V L D + 2 V D + 528 L D + L d_in D + 2228224) floats plus the
+ * weight-image scratch of the forward's bound. */
+RGNN_API int rgnn_rgat_backward(const rgnn_plan_t* plan, const float* node_embeddings, int32_t d_in, int32_t d_out,
+                       const float* const* edge_weights, const float* const* attention, int num_heads, int activation,
+                       const float* grad_out, float* grad_node_embeddings, float* const* grad_edge_weights,
+                       float* const* grad_attention, void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- gnns/gnn_film.py:8-122  sparse_gnn_film_layer -----------------------------------------
  * film_weights: L pointers, kernel [d_in, 2*d_out] (gamma = cols [0,d), beta = cols [d,2d)).

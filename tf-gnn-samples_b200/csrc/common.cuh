@@ -102,6 +102,22 @@ __device__ __forceinline__ float4 act4_cold(float4 v, int act) {
   if (act == RGNN_ACT_LINEAR) return v;
   return slow_act4(v, act);
 }
+// d act(x) / dx from the pre-activation x (utils/utils.py:36-58); transcendental cases out of line, as above
+static __device__ __noinline__ float act_grad_slow(float x, int act) {
+  switch (act) {
+    case RGNN_ACT_TANH: { const float y = fast_tanh(x); return 1.0f - y * y; }
+    case RGNN_ACT_ELU: return x > 0.0f ? 1.0f : expf(x);
+    case RGNN_ACT_SELU: return x > 0.0f ? 1.0507009873554805f : 1.0507009873554805f * 1.6732632423543772f * expf(x);
+    case RGNN_ACT_GELU: return 0.5f * (1.0f + erff(x * 0.70710678118654752f)) + x * 0.3989422804014327f * expf(-0.5f * x * x);
+    default: return 1.0f;
+  }
+}
+__device__ __forceinline__ float act_grad(float x, int act) {
+  if (act == RGNN_ACT_LINEAR) return 1.0f;
+  if (act == RGNN_ACT_RELU) return x > 0.0f ? 1.0f : 0.0f;
+  if (act == RGNN_ACT_LEAKY_RELU) return x > 0.0f ? 1.0f : 0.2f;
+  return act_grad_slow(x, act);
+}
 
 // Programmatic dependent launch (sm_90+): a kernel launched with cudaLaunchAttributeProgrammaticStreamSerialization may
 // become resident while its predecessor in the stream is still running; pdl_wait() blocks until the predecessor grid has

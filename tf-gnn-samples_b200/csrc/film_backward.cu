@@ -25,22 +25,6 @@ __device__ __forceinline__ float4 mul4(float4 a, float4 b) { return make_float4(
 __device__ __forceinline__ float4 scl4(float4 a, float s) { return make_float4(a.x * s, a.y * s, a.z * s, a.w * s); }
 __device__ __forceinline__ void st4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
 
-// d act(x) / dx from the pre-activation x (utils/utils.py:36-58); transcendental cases out of line, as in common.cuh
-static __device__ __noinline__ float act_grad_slow(float x, int act) {
-  switch (act) {
-    case RGNN_ACT_TANH: { const float y = fast_tanh(x); return 1.0f - y * y; }
-    case RGNN_ACT_ELU: return x > 0.0f ? 1.0f : expf(x);
-    case RGNN_ACT_SELU: return x > 0.0f ? 1.0507009873554805f : 1.0507009873554805f * 1.6732632423543772f * expf(x);
-    case RGNN_ACT_GELU: return 0.5f * (1.0f + erff(x * 0.70710678118654752f)) + x * 0.3989422804014327f * expf(-0.5f * x * x);
-    default: return 1.0f;
-  }
-}
-__device__ __forceinline__ float act_grad(float x, int act) {
-  if (act == RGNN_ACT_LINEAR) return 1.0f;
-  if (act == RGNN_ACT_RELU) return x > 0.0f ? 1.0f : 0.0f;
-  if (act == RGNN_ACT_LEAKY_RELU) return x > 0.0f ? 1.0f : 0.2f;
-  return act_grad_slow(x, act);
-}
 // g = act'(gamma * st + beta) * d_a, element-wise
 __device__ __forceinline__ float4 edge_grad(float4 gm, float4 st, float4 bt, float4 da, int act) {
   return make_float4(act_grad(gm.x * st.x + bt.x, act) * da.x, act_grad(gm.y * st.y + bt.y, act) * da.y,

@@ -324,6 +324,11 @@ extern "C" size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, 
       floats = 6 * V * L * dd + V * (dd + di) + (size_t)FILM_LN_MAX_BLOCKS * 2 * dd + (RGNN_WAVE_SMS * 16384 + 2 * L * di * dd) + 64 * 1024;
       break;
     }
+    case RGNN_LAYER_RGAT_BACKWARD: {   // T, dT [V, L, D]; s_src, s_tgt, D_src, D_tgt [<= V, L, K]; d_o [Vt, D]; m, den, c [Vt, K]
+      const size_t di = (size_t)d_in, dd = (size_t)d_out;   // (K <= D / 4); d_att partials; split-K tiles of d_W
+      floats = 3 * V * L * dd + 2 * V * dd + (size_t)RGAT_ATT_MAX_BLOCKS * L * 2 * dd + (RGNN_WAVE_SMS * 16384 + L * di * dd) + 64 * 1024;
+      break;
+    }
     default: return 0;
   }
   // scratch for the pre-swizzled hi/lo weight images of the largest dense contraction of the layer
@@ -669,6 +674,110 @@ extern "C" int rgnn_rgat_forward(const rgnn_plan_t* plan, const float* h, int32_
     RGNN_PROPAGATE(launch_seg_rgat(r, stream));                                                      // rgat.py:120-138
     cur = dst; din = D;
   }
+  return RGNN_OK;
+}
+
+// Backward of ONE timestep of sparse_rgat_layer: what tf.gradients produces for gnns/rgat.py:83-139.  No forward state is
+// kept: the tables are recomputed (rgat_backward.cu has the math).
+//   T = h . [W_0|..|W_{L-1}] (V rows), s_src / s_tgt = per-head scores of T (rgat_scores_kernel)
+//   target side (CSR by target): softmax statistics, d_o = act'(o) grad_out, c, D_tgt      source side (reverse index): dT, D_src
+//   d_att_l = [sum_u D_src T | sum_{v<Vt} D_tgt T] per head           per-CTA partials, fixed-order sum
+//   d_h = dT . [W_l]^T (V rows)   transposed-image GEMM;   d_W_l = h^T . dT[:, l, :]   TN GEMM, split-K, deterministic
+extern "C" int rgnn_rgat_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d_in, int32_t d_out,
+                                  const float* const* edge_weights, const float* const* attention, int num_heads, int activation,
+                                  const float* grad_out, float* grad_h, float* const* grad_edge_weights,
+                                  float* const* grad_attention, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  rgnn_plan* plan = const_cast<rgnn_plan*>(plan_c);   // the reverse index is built lazily inside the plan
+  RGNN_REQUIRE(plan != nullptr, "rgat_backward: plan is NULL");
+  RGNN_REQUIRE(h != nullptr, "rgat_backward: node_embeddings is NULL");
+  RGNN_REQUIRE(edge_weights != nullptr, "rgat_backward: edge_weights is NULL");
+  RGNN_REQUIRE(attention != nullptr, "rgat_backward: attention is NULL");
+  RGNN_REQUIRE(grad_out != nullptr, "rgat_backward: grad_out is NULL");
+  RGNN_REQUIRE(d_in > 0 && d_out > 0 && (d_in % 4) == 0 && (d_out % 4) == 0,
+               "rgat_backward: d_in / d_out must be positive multiples of 4 (d_in=%d, d_out=%d)", d_in, d_out);
+  if (d_out > RGNN_MAX_STATE_DIM) {
+    set_error("rgat_backward: d_out %d > %d (a warp holds a whole row) is not supported", d_out, RGNN_MAX_STATE_DIM);
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_REQUIRE(num_heads >= 1 && (d_out % num_heads) == 0, "rgat_backward: num_heads %d does not divide d_out %d", num_heads, d_out);
+  if (((d_out / num_heads) % 4) != 0) {
+    set_error("rgat_backward: per-head dim %d (d_out %d / num_heads %d) must be a multiple of 4", d_out / num_heads, d_out, num_heads);
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_PROPAGATE(check_act(activation, "rgat_backward"));
+  RGNN_REQUIRE(aligned16(h) && aligned16(grad_out) && aligned16(grad_h),
+               "rgat_backward: node_embeddings / grad_out / grad_node_embeddings must be 16-byte aligned");
+  RGNN_REQUIRE(grad_h != h, "rgat_backward: grad_node_embeddings must not alias node_embeddings");
+  const int V = plan->V, Vt = plan->Vt, L = plan->L, D = d_out, K = num_heads;
+  RgatBwdParams ep;
+  RgatAttOut att_out;
+  for (int l = 0; l < L; ++l) {
+    RGNN_REQUIRE(edge_weights[l] != nullptr, "rgat_backward: edge weight %d is NULL", l);
+    RGNN_REQUIRE(attention[l] != nullptr && aligned16(attention[l]), "rgat_backward: attention vector %d is NULL / misaligned", l);
+    RGNN_REQUIRE(grad_edge_weights == nullptr || (grad_edge_weights[l] != nullptr && aligned16(grad_edge_weights[l])),
+                 "rgat_backward: grad edge weight %d is NULL / misaligned", l);
+    RGNN_REQUIRE(grad_attention == nullptr || grad_attention[l] != nullptr, "rgat_backward: grad attention %d is NULL", l);
+    ep.att.att[l] = attention[l];
+    att_out.ptr[l] = grad_attention != nullptr ? grad_attention[l] : nullptr;
+  }
+
+  // every carve-out and the largest weight-image scratch of the two dense contractions, before anything is enqueued
+  Arena ar(workspace, workspace_bytes);
+  float* T = ar.floats((size_t)V * L * D);
+  float* dT = ar.floats((size_t)V * L * D);
+  float* ssrc = ar.floats((size_t)V * L * K);
+  float* stgt = ar.floats((size_t)V * L * K);
+  float* dsrc = ar.floats((size_t)V * L * K);
+  float* dtgt = ar.floats((size_t)Vt * L * K);
+  float* d_o = ar.floats((size_t)Vt * D);
+  float* stats = ar.floats((size_t)3 * Vt * K);
+  float* att_part = grad_attention != nullptr ? ar.floats((size_t)rgat_att_blocks(V) * L * 2 * D + 4) : nullptr;
+  float* tn_scratch = grad_edge_weights != nullptr ? ar.floats(gemm_tn_scratch_floats(d_in, L * D, V)) : nullptr;
+  GemmParams gT, gH;
+  gT.A1 = h; gT.lda1 = d_in; gT.K1 = d_in; gT.M = V; gT.N = D; gT.C = T; gT.ldc = L * D; gT.ldb1 = D;
+  gT.batch_mode = BATCH_SHARED_A; gT.batch = L;
+  gH.A1 = dT; gH.lda1 = L * D; gH.K1 = L * D; gH.M = V; gH.N = d_in; gH.C = grad_h; gH.ldc = d_in; gH.ldb1 = D;
+  gH.batch_mode = BATCH_K_BLOCKS_T; gH.batch = L; gH.k_block = D;
+  for (int l = 0; l < L; ++l) {
+    gT.bptr[l] = edge_weights[l]; gH.bptr[l] = edge_weights[l];
+    gT.bptr2[l] = gH.bptr2[l] = nullptr;
+  }
+  size_t pack = gemm_tc_pack_bytes(gT);
+  if (grad_h != nullptr) pack = std::max(pack, gemm_tc_pack_bytes(gH));
+  {
+    const size_t mark = ar.used;
+    ar.floats(pack / sizeof(float));
+    RGNN_PROPAGATE(check_ws(ar, "rgat_backward"));
+    ar.used = mark;
+  }
+  RGNN_PROPAGATE(plan_ensure_reverse(plan, stream));
+  RGNN_PROPAGATE(plan_wait_sources(plan, stream));   // T reads the halo rows
+
+  // forward tables: T and the per-head scores (every head width)
+  if (V > 0) {
+    RGNN_PROPAGATE(run_gemm(gT, ar, stream));
+    RGNN_PROPAGATE(launch_rgat_scores(T, V, L, D, K, ep.att, ssrc, stgt, stream));
+  }
+  ep.V = V; ep.Vt = Vt; ep.L = L; ep.D = D; ep.K = K; ep.act = activation;
+  ep.seg_off = plan->seg_off; ep.e_src = plan->e_src; ep.e_type = plan->e_type;
+  ep.heavy_list = plan->heavy_list; ep.heavy_count = plan->err_flag + 1;
+  ep.rev_off = plan->rev_seg_off; ep.rev_tgt = plan->rev_src;
+  ep.rev_heavy_list = plan->rev_heavy_list; ep.rev_heavy_count = plan->err_flag + 2;
+  ep.T = T; ep.s_src = ssrc; ep.s_tgt = stgt; ep.grad_out = grad_out;
+  ep.d_o = d_o; ep.stat_m = stats; ep.stat_den = stats + (size_t)Vt * K; ep.stat_c = stats + (size_t)2 * Vt * K;
+  ep.D_tgt = dtgt; ep.D_src = dsrc; ep.dT = dT;
+  RGNN_PROPAGATE(launch_rgat_edge_backward(ep, plan->num_heavy_host, stream));
+
+  // the outputs, each written once
+  if (grad_attention != nullptr) RGNN_PROPAGATE(launch_rgat_att_backward(ep, att_part, att_out, stream));
+  if (grad_edge_weights != nullptr) {
+    GemmTnOut tn;
+    tn.block_cols = D; tn.ld = D;
+    for (int l = 0; l < L; ++l) tn.ptr[l] = grad_edge_weights[l];
+    RGNN_PROPAGATE(launch_gemm_tn(h, d_in, dT, L * D, d_in, L * D, V, tn, tn_scratch, stream));
+  }
+  if (grad_h != nullptr && V > 0) RGNN_PROPAGATE(run_gemm(gH, ar, stream));
   return RGNN_OK;
 }
 

@@ -147,4 +147,36 @@ int launch_film_edge_backward(const FilmBwdParams& p, int heavy_known, cudaStrea
 // y[0:n] += x[0:n]  (n % 4 == 0)
 int launch_add_rows(float* y, const float* x, long n, cudaStream_t stream);
 
+// ---- rgnn_rgat_backward (rgat_backward.cu) ----
+// The edge kernels: d_o [Vt, D], the softmax statistics m / den / c [Vt, K] and D_tgt [Vt, L, K] over the CSR by target;
+// dT [V, L, D] and D_src [V, L, K] over the reverse index.
+struct RgatBwdParams {
+  int V = 0, Vt = 0, L = 1, D = 0, K = 1, act = RGNN_ACT_LINEAR;
+  AttnTable att;                       // per-type attention vectors [2D]
+  const int32_t* seg_off = nullptr; const int32_t* e_src = nullptr; const int32_t* e_type = nullptr;
+  const int32_t* heavy_list = nullptr; const int* heavy_count = nullptr;          // targets above RGNN_HEAVY_SEGMENT
+  const int32_t* rev_off = nullptr; const int32_t* rev_tgt = nullptr;             // segment u * L + l, entry = target
+  const int32_t* rev_heavy_list = nullptr; const int* rev_heavy_count = nullptr;
+  const float* T = nullptr;            // [V, L, D]   h . [W_0 | .. | W_{L-1}]
+  const float* s_src = nullptr;        // [V, L, K]
+  const float* s_tgt = nullptr;        // [V, L, K]
+  const float* grad_out = nullptr;     // [Vt, D]
+  float* d_o = nullptr;                // [Vt, D]    act'(o) * grad_out
+  float* stat_m = nullptr;             // [Vt, K]    softmax max
+  float* stat_den = nullptr;           // [Vt, K]    softmax denominator
+  float* stat_c = nullptr;             // [Vt, K]    <d_o, o> per head
+  float* D_tgt = nullptr;              // [Vt, L, K] sum of d_x over the (target, type) run
+  float* D_src = nullptr;              // [V, L, K]  sum of d_x over the (source, type) segment
+  float* dT = nullptr;                 // [V, L, D]
+};
+int launch_rgat_edge_backward(const RgatBwdParams& p, int heavy_known, cudaStream_t stream);
+// d_att_l [2D] from T, D_src and D_tgt: per-CTA partial sums in partial [rgat_att_blocks(V), L, 2D], added in CTA order
+struct RgatAttOut { float* ptr[RGNN_MAX_EDGE_TYPES]; };
+constexpr int RGAT_ATT_MAX_BLOCKS = 2 * RGNN_WAVE_SMS;
+inline int rgat_att_blocks(int V) {
+  const int b = (V + 63) / 64;
+  return b < RGAT_ATT_MAX_BLOCKS ? b : RGAT_ATT_MAX_BLOCKS;
+}
+int launch_rgat_att_backward(const RgatBwdParams& p, float* partial, const RgatAttOut& out, cudaStream_t stream);
+
 }  // namespace rgnn

@@ -57,6 +57,8 @@ SIGNATURES = {
                                   _PTR, _PTR, c_size_t, _PTR]),
     "rgnn_film_backward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, _PTR, _PTR, _PTR, c_int, c_int, c_int, _PTR, _PTR,
                                    _PTR, _PTR, _PTR, _PTR, _PTR, c_size_t, _PTR]),
+    "rgnn_rgat_backward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, c_int, c_int, _PTR, _PTR, _PTR, _PTR, _PTR, c_size_t,
+                                   _PTR]),
     "rgnn_edge_mlp_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, c_int, _PTR, _PTR, _PTR,
                                       c_int, c_int, c_int, c_int, c_int, _PTR, _PTR, c_size_t, _PTR]),
     "rgnn_rgin_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, c_int, _PTR, _PTR, c_int, _PTR, _PTR,
