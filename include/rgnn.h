@@ -24,8 +24,8 @@
  *             rgnn_set_weight_cache(0) call cudaFree: never call them during a capture.
  *   capture   run eagerly once before capturing: every layer with the weight cache on (a cache miss
  *             during capture is an error), and the first backward on a plan (rgnn_rgcn_backward /
- *             rgnn_film_backward / rgnn_rgat_backward / rgnn_edge_aggregate_backward build the plan's reverse index then;
- *             inside a capture they
+ *             rgnn_film_backward / rgnn_rgat_backward / rgnn_ggnn_backward / rgnn_edge_aggregate_backward build the plan's
+ *             reverse index then; inside a capture they
  *             return RGNN_E_INVALID).  A plan built with RGNN_PLAN_DEFERRED_CHECK inside a capture is
  *             filled only when the graph is replayed: call rgnn_plan_status after a replay.  A graph
  *             captured with the weight cache on reads the cached images: rgnn_weight_cache_clear (and
@@ -85,7 +85,7 @@ enum rgnn_layer_kind {
   RGNN_LAYER_RGCN = 0, RGNN_LAYER_GGNN = 1, RGNN_LAYER_RGAT = 2, RGNN_LAYER_FILM = 3,
   RGNN_LAYER_EDGE_MLP = 4, RGNN_LAYER_RGIN = 5, RGNN_LAYER_RGCN_BACKWARD = 6,
   RGNN_LAYER_RGDCN = 7,  /* rgnn_workspace_bytes: pass channel_dim as mlp_layers */
-  RGNN_LAYER_FILM_BACKWARD = 8, RGNN_LAYER_RGAT_BACKWARD = 9
+  RGNN_LAYER_FILM_BACKWARD = 8, RGNN_LAYER_RGAT_BACKWARD = 9, RGNN_LAYER_GGNN_BACKWARD = 10
 };
 
 typedef struct rgnn_plan rgnn_plan_t;
@@ -196,6 +196,29 @@ RGNN_API int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* node_embedd
                       const float* cell_recurrent_kernel, const float* cell_bias,
                       int cell_kind, int activation, int aggregation, int num_timesteps,
                       float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of ONE timestep of sparse_ggnn_layer (ggnn.py:76-93, Keras TF-1.13 GRU / SimpleRNN cell): the gradients
+ * TensorFlow autodiff produces.  Gradients are written, not accumulated.  No forward state is needed: the call recomputes the
+ * aggregate m and the cell's pre-activations from its inputs, and builds no per-edge tensor.
+ *   node_embeddings [V, d]: this timestep's INPUT; weights as rgnn_ggnn_forward (cell_bias 16-byte aligned too)
+ *   grad_out [num_targets, d] (rows [0, num_targets) of the plan, rgnn_plan_set_num_targets)
+ *   grad_node_embeddings [V, d] covers EVERY local row (halo rows included: what rgnn_halo_exchange_backward consumes) or
+ *   NULL, and must not alias node_embeddings or grad_out; grad_edge_weights: host array of L device pointers [d, d] or NULL;
+ *   grad_cell_kernel / grad_cell_recurrent_kernel [d, 3d] (GRU) / [d, d] (RNN) or NULL; grad_cell_bias [3d] / [d] or NULL.
+ * 'max' aggregation: RGNN_E_UNSUPPORTED.  Every argument is checked and the workspace sized before anything is enqueued.
+ * The first backward on a plan builds its reverse index (as rgnn_rgcn_backward; not inside a capture).  Two identical calls
+ * are bit-identical (no atomics: every output has one writer, every sum a fixed order).
+ * Several timesteps are the caller's loop: run the forward with num_timesteps = 1 per timestep keeping each input, call
+ * this from the last timestep down (grad_out of step t = grad_node_embeddings of step t + 1), and add the shared weights'
+ * gradients of the steps.
+ * Workspace: rgnn_workspace_bytes(plan, RGNN_LAYER_GGNN_BACKWARD, d, d, 0): with V = num_nodes, L = num_edge_types,
+ * (V L d + 11 V d + 792 d + (L + 3) d^2 + 2228224) floats plus the weight-image scratch of the forward's bound. */
+RGNN_API int rgnn_ggnn_backward(const rgnn_plan_t* plan, const float* node_embeddings, int32_t d,
+                       const float* const* edge_weights, const float* cell_kernel, const float* cell_recurrent_kernel,
+                       const float* cell_bias, int cell_kind, int activation, int aggregation,
+                       const float* grad_out, float* grad_node_embeddings, float* const* grad_edge_weights,
+                       float* grad_cell_kernel, float* grad_cell_recurrent_kernel, float* grad_cell_bias,
+                       void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- gnns/rgat.py:9-141  sparse_rgat_layer -------------------------------------------------
  * attention: host array of L device pointers [2 * d_out]; head k uses [k*2d, (k+1)*2d),

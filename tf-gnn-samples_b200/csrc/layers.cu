@@ -142,6 +142,17 @@ int transform_sources(const rgnn_plan_t* plan, Arena& ar, const float* cur, int 
   s.table = T; s.stride_idx = (long)L * D; s.stride_type = D;
   return RGNN_OK;
 }
+// the weight-image scratch transform_sources() takes from the arena (sized before anything is enqueued)
+size_t transform_sources_pack_bytes(const rgnn_plan_t* plan, int d_in, int D) {
+  GemmParams g;
+  g.K1 = d_in; g.N = D; g.batch = plan->L;
+  if (plan->n_pairs >= 0 && plan->pair_src != nullptr) {
+    g.batch_mode = BATCH_ROW_RANGES; g.M = plan->n_pairs; g.max_rows = plan->max_type_pairs;
+  } else {
+    g.batch_mode = BATCH_SHARED_A; g.M = plan->V;
+  }
+  return gemm_tc_pack_bytes(g);
+}
 
 // scratch for the multi-CTA split of heavy targets (seg_kernels.cu); nothing when the plan is known to have none
 size_t heavy_scratch_floats(const rgnn_plan_t* plan, size_t d) {
@@ -327,6 +338,11 @@ extern "C" size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, 
     case RGNN_LAYER_RGAT_BACKWARD: {   // T, dT [V, L, D]; s_src, s_tgt, D_src, D_tgt [<= V, L, K]; d_o [Vt, D]; m, den, c [Vt, K]
       const size_t di = (size_t)d_in, dd = (size_t)d_out;   // (K <= D / 4); d_att partials; split-K tiles of d_W
       floats = 3 * V * L * dd + 2 * V * dd + (size_t)RGAT_ATT_MAX_BLOCKS * L * 2 * dd + (RGNN_WAVE_SMS * 16384 + L * di * dd) + 64 * 1024;
+      break;
+    }
+    case RGNN_LAYER_GGNN_BACKWARD: {   // T, then dT [V, L, D]; m, dm [V, D]; a, da [Vt, 3D]; rh, d(rh) / f, e [Vt, D];
+      const size_t dd = (size_t)d_out;   // bias partials; split-K tiles of d_W / d_K / d_R
+      floats = V * L * dd + 11 * V * dd + (size_t)GGNN_COLSUM_MAX_BLOCKS * 3 * dd + (RGNN_WAVE_SMS * 16384 + (L + 3) * dd * dd) + 64 * 1024;
       break;
     }
     default: return 0;
@@ -627,6 +643,183 @@ extern "C" int rgnn_ggnn_forward(const rgnn_plan_t* plan, const float* h, int32_
       }
     }
     cur = dst;
+  }
+  return RGNN_OK;
+}
+
+// Backward of ONE timestep of sparse_ggnn_layer: what tf.gradients produces for gnns/ggnn.py:76-93.  No forward state is
+// kept: m and the cell's pre-activations are recomputed (ggnn_backward.cu has the element-wise math).
+//   T = h . [W_0|..|W_{L-1}], m = agg T (transform_sources + segment reduce, as the forward)
+//   GRU: [a_z|a_r] = [m|h] . [K_zr;R_zr] + b_zr,  rh = r h,  a_h = [m|rh] . [K_h;R_h] + b_h       (wgmma GEMM, A2 = 2nd operand)
+//        da_z, da_h, e = g z;  d(rh) = da_h . R_h^T;  da_r, e += d(rh) r;  f = [da_z|da_r] . R_zr^T
+//   RNN: a = [m|h] . [K;R] + b;  da = g act'(a);  f = da . R^T
+//   dm = da . K^T (/ div(v); rows >= Vt are zero),  dT[u,l] = sum_{(u->v) in A_l} dm[v]   (reverse index; dT reuses T)
+//   d_h = dT . [W_l]^T (V rows), then rows < Vt += e + f          d_W_l = h^T . dT[:, l, :]
+//   d_K = m^T . da,  d_R = h^T . [da_z|da_r] | rh^T . da_h  (RNN: h^T . da),  d_b = column sums of da (CTA partials, fixed order)
+extern "C" int rgnn_ggnn_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d, const float* const* edge_weights,
+                                  const float* cell_kernel, const float* cell_recurrent_kernel, const float* cell_bias,
+                                  int cell_kind, int activation, int aggregation, const float* grad_out, float* grad_h,
+                                  float* const* grad_edge_weights, float* grad_cell_kernel,
+                                  float* grad_cell_recurrent_kernel, float* grad_cell_bias, void* workspace,
+                                  size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  rgnn_plan* plan = const_cast<rgnn_plan*>(plan_c);   // the reverse index is built lazily inside the plan
+  RGNN_REQUIRE(plan != nullptr, "ggnn_backward: plan is NULL");
+  RGNN_REQUIRE(h != nullptr, "ggnn_backward: node_embeddings is NULL");
+  RGNN_REQUIRE(edge_weights != nullptr, "ggnn_backward: edge_weights is NULL");
+  RGNN_REQUIRE(cell_kernel != nullptr, "ggnn_backward: cell_kernel is NULL");
+  RGNN_REQUIRE(cell_recurrent_kernel != nullptr, "ggnn_backward: cell_recurrent_kernel is NULL");
+  RGNN_REQUIRE(cell_bias != nullptr, "ggnn_backward: cell_bias is NULL");
+  RGNN_REQUIRE(grad_out != nullptr, "ggnn_backward: grad_out is NULL");
+  RGNN_REQUIRE(d > 0 && (d % 4) == 0, "ggnn_backward: state dim d must be a positive multiple of 4 (d=%d)", d);
+  RGNN_REQUIRE(cell_kind == RGNN_CELL_RNN || cell_kind == RGNN_CELL_GRU, "ggnn_backward: Unknown RNN cell type code %d", cell_kind);
+  RGNN_PROPAGATE(check_act(activation, "ggnn_backward"));
+  RGNN_PROPAGATE(check_agg(aggregation, "ggnn_backward"));
+  if (aggregation == RGNN_AGG_MAX) {
+    set_error("ggnn_backward: the gradient of 'max' aggregation is not implemented in this build");
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_REQUIRE(aligned16(h) && aligned16(grad_out), "ggnn_backward: node_embeddings / grad_out must be 16-byte aligned");
+  RGNN_REQUIRE(aligned16(cell_kernel) && aligned16(cell_recurrent_kernel) && aligned16(cell_bias),
+               "ggnn_backward: cell_kernel / cell_recurrent_kernel / cell_bias must be 16-byte aligned");
+  RGNN_REQUIRE(aligned16(grad_h) && aligned16(grad_cell_kernel) && aligned16(grad_cell_recurrent_kernel) && aligned16(grad_cell_bias),
+               "ggnn_backward: grad_node_embeddings / grad_cell_kernel / grad_cell_recurrent_kernel / grad_cell_bias must be 16-byte aligned");
+  RGNN_REQUIRE(grad_h == nullptr || (grad_h != h && grad_h != grad_out),
+               "ggnn_backward: grad_node_embeddings must not alias node_embeddings or grad_out");
+  const int V = plan->V, Vt = plan->Vt, L = plan->L, D = d;
+  const bool gru = cell_kind == RGNN_CELL_GRU;
+  const int G = gru ? 3 : 1;   // gates
+  for (int l = 0; l < L; ++l) {
+    RGNN_REQUIRE(edge_weights[l] != nullptr, "ggnn_backward: edge weight %d is NULL", l);
+    RGNN_REQUIRE(grad_edge_weights == nullptr || (grad_edge_weights[l] != nullptr && aligned16(grad_edge_weights[l])),
+                 "ggnn_backward: grad edge weight %d is NULL / misaligned", l);
+  }
+
+  // every carve-out and the largest weight-image scratch of the dense contractions, before anything is enqueued
+  Arena ar(workspace, workspace_bytes);
+  float* T = ar.floats((size_t)V * L * D);                   // T, then dT
+  float* m = ar.floats((size_t)Vt * D);
+  float* dm = ar.floats((size_t)V * D);
+  float* a = ar.floats((size_t)Vt * G * D);                  // pre-activations
+  float* da = gru ? ar.floats((size_t)Vt * G * D) : a;       // the RNN backward overwrites a with da
+  float* rh = gru ? ar.floats((size_t)Vt * D) : nullptr;
+  float* f = ar.floats((size_t)Vt * D);                      // GRU: d(rh), then the R_zr term of d_h; RNN: da . R^T
+  float* e = (gru && grad_h != nullptr) ? ar.floats((size_t)Vt * D) : nullptr;
+  float* b_part = grad_cell_bias != nullptr ? ar.floats((size_t)ggnn_colsum_blocks(Vt) * G * D + 4) : nullptr;
+  float* tn_scratch = nullptr;
+  if (grad_edge_weights != nullptr || grad_cell_kernel != nullptr || grad_cell_recurrent_kernel != nullptr) {
+    size_t n = gemm_tn_scratch_floats(D, G * D, Vt);
+    n = std::max(n, gemm_tn_scratch_floats(D, L * D, V));
+    if (gru) n = std::max(n, std::max(gemm_tn_scratch_floats(D, 2 * D, Vt), gemm_tn_scratch_floats(D, D, Vt)));
+    tn_scratch = ar.floats(n);
+  }
+  SegParams heavy;
+  seg_heavy_scratch(heavy, plan, ar, D);
+
+  // the dense contractions
+  GemmParams gA, gAh, gRh, gM, gF, gH;
+  gA.A1 = m; gA.lda1 = D; gA.K1 = D; gA.A2 = h; gA.lda2 = D; gA.K2 = D;           // [a_z|a_r] (GRU) / a (RNN)
+  gA.B1 = cell_kernel; gA.ldb1 = G * D; gA.B2 = cell_recurrent_kernel; gA.ldb2 = G * D;
+  gA.M = Vt; gA.N = gru ? 2 * D : D; gA.bias = cell_bias; gA.C = a; gA.ldc = G * D;
+  gAh = gA;                                                                      // a_h = [m|rh] . [K_h;R_h] + b_h
+  gAh.A2 = rh; gAh.B1 = cell_kernel + 2 * D; gAh.B2 = cell_recurrent_kernel + 2 * D; gAh.N = D; gAh.bias = cell_bias + 2 * D;
+  gAh.C = a + 2 * D;
+  gRh.A1 = da + 2 * D; gRh.lda1 = 3 * D; gRh.K1 = D; gRh.M = Vt; gRh.N = D; gRh.C = f; gRh.ldc = D;   // d(rh) = da_h . R_h^T
+  gRh.batch_mode = BATCH_K_BLOCKS_T; gRh.batch = 1; gRh.k_block = D; gRh.bptr[0] = cell_recurrent_kernel + 2 * D; gRh.ldb1 = 3 * D;
+  gRh.bptr2[0] = nullptr;
+  gM.A1 = da; gM.lda1 = G * D; gM.K1 = G * D; gM.M = Vt; gM.N = D; gM.C = dm; gM.ldc = D;          // dm = da . K^T
+  gM.batch_mode = BATCH_K_BLOCKS_T; gM.batch = 1; gM.k_block = G * D; gM.bptr[0] = cell_kernel; gM.ldb1 = G * D;
+  gM.bptr2[0] = nullptr;
+  gF = gM;                                                       // f = [da_z|da_r] . R_zr^T (GRU) / da . R^T (RNN)
+  gF.K1 = gF.k_block = gru ? 2 * D : D; gF.bptr[0] = cell_recurrent_kernel; gF.C = f;
+  gH.A1 = T; gH.lda1 = L * D; gH.K1 = L * D; gH.M = V; gH.N = D; gH.C = grad_h; gH.ldc = D; gH.ldb1 = D;   // dT . [W_l]^T
+  gH.batch_mode = BATCH_K_BLOCKS_T; gH.batch = L; gH.k_block = D;
+  for (int l = 0; l < L; ++l) { gH.bptr[l] = edge_weights[l]; gH.bptr2[l] = nullptr; }
+  size_t pack = transform_sources_pack_bytes(plan, D, D);
+  if (Vt > 0) {
+    pack = std::max(pack, std::max(gemm_tc_pack_bytes(gA), gemm_tc_pack_bytes(gM)));
+    if (gru) pack = std::max(pack, std::max(gemm_tc_pack_bytes(gAh), gemm_tc_pack_bytes(gRh)));
+    if (grad_h != nullptr) pack = std::max(pack, gemm_tc_pack_bytes(gF));
+  }
+  if (grad_h != nullptr && V > 0) pack = std::max(pack, gemm_tc_pack_bytes(gH));
+  {
+    const size_t mark = ar.used;
+    ar.floats(pack / sizeof(float));
+    RGNN_PROPAGATE(check_ws(ar, "ggnn_backward"));
+    ar.used = mark;
+  }
+  RGNN_PROPAGATE(plan_ensure_reverse(plan, stream));
+
+  // forward: m (transform_sources waits for a pending halo exchange), then the cell's pre-activations
+  {
+    SegParams s;
+    seg_from_plan(s, plan);
+    s.D = D;
+    RGNN_PROPAGATE(transform_sources(plan, ar, h, D, D, edge_weights, T, stream, s));
+    s.agg = aggregation; s.out = m; s.ld_out = D; s.heavy_scratch = heavy.heavy_scratch;
+    RGNN_PROPAGATE(launch_seg_reduce(s, stream));
+  }
+  GgnnCellBwdParams cp;
+  cp.rows = Vt; cp.D = D; cp.act = activation; cp.grad_out = grad_out; cp.h = h; cp.a = a; cp.da = da; cp.drh = f; cp.e = e;
+  if (Vt > 0) {
+    RGNN_PROPAGATE(run_gemm(gA, ar, stream));
+    if (gru) {
+      RGNN_PROPAGATE(launch_ggnn_gru_rh(a, h, Vt, D, rh, stream));
+      RGNN_PROPAGATE(run_gemm(gAh, ar, stream));
+      // the cell backward
+      RGNN_PROPAGATE(launch_ggnn_cell_backward(cp, cell_kind, 0, stream));
+      RGNN_PROPAGATE(run_gemm(gRh, ar, stream));
+      RGNN_PROPAGATE(launch_ggnn_cell_backward(cp, cell_kind, 1, stream));
+    } else {
+      RGNN_PROPAGATE(launch_ggnn_cell_backward(cp, cell_kind, 0, stream));
+    }
+    RGNN_PROPAGATE(run_gemm(gM, ar, stream));
+  }
+  // the edge stage: dT[u, l] = sum over the edges (u -> v) of type l of dm[v]; dT overwrites T
+  RGNN_PROPAGATE(launch_ggnn_dm_finish(dm, V, Vt, D, aggregation, plan->seg_off, stream));
+  {
+    SegParams r;   // reverse index: segment = (source u, type l); gathered row = dm[original target]
+    r.V = V * L; r.L = L; r.D = D;
+    r.seg_off = plan->rev_seg_off; r.e_idx = plan->rev_src; r.e_type = plan->rev_type;
+    r.table = dm; r.stride_idx = D; r.stride_type = 0;
+    r.heavy_list = plan->rev_heavy_list; r.heavy_count = plan->err_flag + 2;
+    r.heavy_threshold = RGNN_HEAVY_SEGMENT; r.heavy_known = -1;
+    r.agg = RGNN_AGG_SUM; r.out = T; r.ld_out = D;
+    RGNN_PROPAGATE(launch_seg_reduce(r, stream));
+  }
+
+  // the outputs, each written once
+  if (grad_edge_weights != nullptr) {
+    GemmTnOut tn;
+    tn.block_cols = D; tn.ld = D;
+    for (int l = 0; l < L; ++l) tn.ptr[l] = grad_edge_weights[l];
+    RGNN_PROPAGATE(launch_gemm_tn(h, D, T, L * D, D, L * D, V, tn, tn_scratch, stream));
+  }
+  if (grad_cell_kernel != nullptr) {
+    GemmTnOut tn;
+    tn.block_cols = G * D; tn.ld = G * D; tn.ptr[0] = grad_cell_kernel;
+    RGNN_PROPAGATE(launch_gemm_tn(m, D, da, G * D, D, G * D, Vt, tn, tn_scratch, stream));
+  }
+  if (grad_cell_recurrent_kernel != nullptr) {
+    GemmTnOut tn;
+    tn.ld = G * D;
+    if (gru) {
+      tn.block_cols = 2 * D; tn.ptr[0] = grad_cell_recurrent_kernel;
+      RGNN_PROPAGATE(launch_gemm_tn(h, D, da, 3 * D, D, 2 * D, Vt, tn, tn_scratch, stream));
+      tn.block_cols = D; tn.ptr[0] = grad_cell_recurrent_kernel + 2 * D;
+      RGNN_PROPAGATE(launch_gemm_tn(rh, D, da + 2 * D, 3 * D, D, D, Vt, tn, tn_scratch, stream));
+    } else {
+      tn.block_cols = D; tn.ptr[0] = grad_cell_recurrent_kernel;
+      RGNN_PROPAGATE(launch_gemm_tn(h, D, da, D, D, D, Vt, tn, tn_scratch, stream));
+    }
+  }
+  if (grad_cell_bias != nullptr) RGNN_PROPAGATE(launch_ggnn_bias_grad(da, Vt, G * D, b_part, grad_cell_bias, stream));
+  if (grad_h != nullptr) {
+    if (V > 0) RGNN_PROPAGATE(run_gemm(gH, ar, stream));
+    if (Vt > 0) {
+      RGNN_PROPAGATE(run_gemm(gF, ar, stream));
+      RGNN_PROPAGATE(launch_ggnn_add_cell_grad(grad_h, gru ? e : f, gru ? f : nullptr, (long)Vt * D, stream));
+    }
   }
   return RGNN_OK;
 }

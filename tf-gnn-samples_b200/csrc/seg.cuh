@@ -179,4 +179,32 @@ inline int rgat_att_blocks(int V) {
 }
 int launch_rgat_att_backward(const RgatBwdParams& p, float* partial, const RgatAttOut& out, cudaStream_t stream);
 
+// ---- rgnn_ggnn_backward (ggnn_backward.cu) ----
+// The element-wise parts of the cell backward over the wanted target rows [0, rows).  GRU: a / da [rows, 3D] hold
+// [a_z | a_r | a_h] / [da_z | da_r | da_h]; stage 0 writes da_z, da_h and e = g z, stage 1 (after d(rh) = da_h . R_h^T) writes
+// da_r and adds d(rh) r to e.  RNN: a / da [rows, D] (da may be a).  e may be NULL (no d_h wanted).
+struct GgnnCellBwdParams {
+  int rows = 0, D = 0, act = RGNN_ACT_LINEAR;
+  const float* grad_out = nullptr;     // [rows, D]
+  const float* h = nullptr;            // [rows, D]  this timestep's input
+  const float* a = nullptr;            // pre-activations
+  float* da = nullptr;
+  const float* drh = nullptr;          // [rows, D]  GRU stage 1
+  float* e = nullptr;                  // [rows, D]  element-wise terms of the cell's d_h
+};
+int launch_ggnn_cell_backward(const GgnnCellBwdParams& p, int cell_kind, int stage, cudaStream_t stream);
+// rh [rows, D] = hs(a_r) * h, a [rows, 3D]
+int launch_ggnn_gru_rh(const float* a, const float* h, int rows, int D, float* rh, cudaStream_t stream);
+// dm [V, D]: rows < Vt divided by the mean / sqrt_n divisor, rows >= Vt zeroed
+int launch_ggnn_dm_finish(float* dm, int V, int Vt, int D, int agg, const int32_t* seg_off, cudaStream_t stream);
+// y[0:n] += e[0:n] + f[0:n] (f may be NULL)
+int launch_ggnn_add_cell_grad(float* y, const float* e, const float* f, long n, cudaStream_t stream);
+// out [N] = column sums of x [rows, N]: per-CTA partial sums in partial [ggnn_colsum_blocks(rows), N], added in CTA order
+constexpr int GGNN_COLSUM_MAX_BLOCKS = 2 * RGNN_WAVE_SMS;
+inline int ggnn_colsum_blocks(int rows) {
+  const int b = (rows + 63) / 64;
+  return b < GGNN_COLSUM_MAX_BLOCKS ? b : GGNN_COLSUM_MAX_BLOCKS;
+}
+int launch_ggnn_bias_grad(const float* x, int rows, int N, float* partial, float* out, cudaStream_t stream);
+
 }  // namespace rgnn

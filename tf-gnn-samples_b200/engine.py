@@ -51,6 +51,8 @@ SIGNATURES = {
                                    _PTR, c_size_t, _PTR]),
     "rgnn_ggnn_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, _PTR, _PTR, c_int, c_int, c_int, c_int,
                                   _PTR, _PTR, c_size_t, _PTR]),
+    "rgnn_ggnn_backward": (c_int, [_PTR, _PTR, c_int32, _PTR, _PTR, _PTR, _PTR, c_int, c_int, c_int, _PTR, _PTR, _PTR, _PTR,
+                                   _PTR, _PTR, _PTR, c_size_t, _PTR]),
     "rgnn_rgat_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, c_int, c_int, c_int,
                                   _PTR, _PTR, c_size_t, _PTR]),
     "rgnn_film_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, _PTR, _PTR, _PTR, _PTR, c_int, c_int, c_int, c_int,
