@@ -24,8 +24,8 @@
  *             rgnn_set_weight_cache(0) call cudaFree: never call them during a capture.
  *   capture   run eagerly once before capturing: every layer with the weight cache on (a cache miss
  *             during capture is an error), and the first backward on a plan (rgnn_rgcn_backward /
- *             rgnn_film_backward / rgnn_rgat_backward / rgnn_ggnn_backward / rgnn_edge_aggregate_backward build the plan's
- *             reverse index then; inside a capture they
+ *             rgnn_film_backward / rgnn_rgat_backward / rgnn_ggnn_backward / rgnn_rgin_backward /
+ *             rgnn_edge_aggregate_backward build the plan's reverse index then; inside a capture they
  *             return RGNN_E_INVALID).  A plan built with RGNN_PLAN_DEFERRED_CHECK inside a capture is
  *             filled only when the graph is replayed: call rgnn_plan_status after a replay.  A graph
  *             captured with the weight cache on reads the cached images: rgnn_weight_cache_clear (and
@@ -85,7 +85,8 @@ enum rgnn_layer_kind {
   RGNN_LAYER_RGCN = 0, RGNN_LAYER_GGNN = 1, RGNN_LAYER_RGAT = 2, RGNN_LAYER_FILM = 3,
   RGNN_LAYER_EDGE_MLP = 4, RGNN_LAYER_RGIN = 5, RGNN_LAYER_RGCN_BACKWARD = 6,
   RGNN_LAYER_RGDCN = 7,  /* rgnn_workspace_bytes: pass channel_dim as mlp_layers */
-  RGNN_LAYER_FILM_BACKWARD = 8, RGNN_LAYER_RGAT_BACKWARD = 9, RGNN_LAYER_GGNN_BACKWARD = 10
+  RGNN_LAYER_FILM_BACKWARD = 8, RGNN_LAYER_RGAT_BACKWARD = 9, RGNN_LAYER_GGNN_BACKWARD = 10,
+  RGNN_LAYER_RGIN_BACKWARD = 11
 };
 
 typedef struct rgnn_plan rgnn_plan_t;
@@ -307,6 +308,35 @@ RGNN_API int rgnn_rgin_forward(const rgnn_plan_t* plan, const float* node_embedd
                       const float* ln_gamma, const float* ln_beta,
                       int activation, int aggregation, int use_target_state_as_input, int num_timesteps,
                       float* out, void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of ONE timestep of sparse_rgin_layer with source-only messages (rgin.py:103-139, use_target_state_as_input = 0:
+ * the default of every reference config): the gradients TensorFlow autodiff produces.  Gradients are written, not
+ * accumulated.  No forward state is needed: the call recomputes the edge MLP on the node rows (a message depends on its
+ * source and type only), the aggregate and the aggregation MLP from its inputs, and builds no per-edge tensor.
+ *   node_embeddings [V, d_in]: this timestep's INPUT; the MLP tables and dims as rgnn_rgin_forward (either MLP may be None,
+ *   with the same width limits); ln_gamma / ln_beta: this timestep's [d_out]
+ *   grad_out [num_targets, d_out] (rows [0, num_targets) of the plan, rgnn_plan_set_num_targets)
+ *   grad_node_embeddings [V, d_in] covers EVERY local row (halo rows included: what rgnn_halo_exchange_backward consumes) or
+ *   NULL, and must not alias node_embeddings or grad_out; grad_edge_mlp_kernels: host array of L * n_e device pointers
+ *   (type-major, as the forward's table) or NULL; grad_aggr_kernels: host array of n_a device pointers or NULL;
+ *   grad_ln_gamma / grad_ln_beta [d_out] or NULL.  (n_e, n_a = number of kernels of the edge / aggregation MLP.)
+ * use_target_state_as_input = 1, 'max' aggregation and d_out > RGNN_MAX_STATE_DIM: RGNN_E_UNSUPPORTED.  Every argument is
+ * checked and the workspace sized before anything is enqueued.  The first backward on a plan builds its reverse index (as
+ * rgnn_rgcn_backward; not inside a capture).  Two identical calls are bit-identical (no atomics: every output has one
+ * writer, every sum a fixed order).
+ * Several timesteps are the caller's loop: run the forward with num_timesteps = 1 per timestep keeping each input, call
+ * this from the last timestep down (grad_out of step t = grad_node_embeddings of step t + 1), and add the shared weights'
+ * gradients of the steps.
+ * Workspace: rgnn_workspace_bytes(plan, RGNN_LAYER_RGIN_BACKWARD, d_in, d_out, max(n_e, n_a)): with V = num_nodes,
+ * L = num_edge_types, dm = max(2 d_in, d_out), nl = max(n_e, n_a, 1),
+ * (2 nl V L dm + (2 nl + 2) V dm + 528 d_out + L dm^2 + 2228224) floats plus the weight-image scratch of the forward's bound. */
+RGNN_API int rgnn_rgin_backward(const rgnn_plan_t* plan, const float* node_embeddings, int32_t d_in, int32_t d_out,
+                       const float* const* edge_mlp_kernels, const int32_t* edge_mlp_dims, int num_edge_mlp_hidden_layers,
+                       const float* const* aggr_kernels, const int32_t* aggr_dims, int num_aggr_mlp_hidden_layers,
+                       const float* ln_gamma, const float* ln_beta, int activation, int aggregation,
+                       int use_target_state_as_input, const float* grad_out, float* grad_node_embeddings,
+                       float* const* grad_edge_mlp_kernels, float* const* grad_aggr_kernels, float* grad_ln_gamma,
+                       float* grad_ln_beta, void* workspace, size_t workspace_bytes, void* stream);
 
 /* gnns/rgdcn.py:8-171 -- relational graph DYNAMIC convolution: the state is split into num_channels channels of
  * K = d / num_channels; message of edge (u -> v, type l), channel c:  h_u[c,:] . W[v,l,c]  with the K x K kernel

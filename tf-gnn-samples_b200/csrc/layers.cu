@@ -345,6 +345,12 @@ extern "C" size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, 
       floats = V * L * dd + 11 * V * dd + (size_t)GGNN_COLSUM_MAX_BLOCKS * 3 * dd + (RGNN_WAVE_SMS * 16384 + (L + 3) * dd * dd) + 64 * 1024;
       break;
     }
+    case RGNN_LAYER_RGIN_BACKWARD: {   // Z_j, A_j and dQ / dA [V, L, <= dm] (at most 2 nl of them); a / d_a [V, dm];
+      const size_t nl = (size_t)(mlp_layers > 0 ? mlp_layers : 1), dd = (size_t)d_out;   // U_k, Y_k, n [Vt <= V, dm];
+      floats = 2 * nl * V * L * dm + (2 * nl + 2) * V * dm + (size_t)FILM_LN_MAX_BLOCKS * 2 * dd   // LN partials;
+               + (RGNN_WAVE_SMS * 16384 + L * dm * dm) + 64 * 1024;                             // split-K tiles of d_E / d_K
+      break;
+    }
     default: return 0;
   }
   // scratch for the pre-swizzled hi/lo weight images of the largest dense contraction of the layer
@@ -1278,6 +1284,273 @@ extern "C" int rgnn_rgin_forward(const rgnn_plan_t* plan, const float* h, int32_
     }
     cur = dst;
   }
+  return RGNN_OK;
+}
+
+// Backward of ONE timestep of sparse_rgin_layer with source-only messages: what tf.gradients produces for gnns/rgin.py:103-139.
+// The message of edge (u -> v, l) depends on (u, l) only, so the edge MLP runs on the V node rows and nothing per edge is
+// built.  No forward state is kept: every table is recomputed (rgin_backward.cu has the element-wise math).
+//   Z_1 = h . [E_{0,1}|..|E_{L-1,1}] (shared-A GEMM), A_j = act(Z_j), Z_{j+1}[:, l] = A_j[:, l] . E_{l,j+1} (column blocks)
+//   a = agg_{(u->v) in A_l} act(Z_{n_e}[u, l]) (segment reduce, Vt rows), U_k = Y_{k-1} . K_k, Y_k = act(U_k), Y_0 = a
+//   dn = LayerNorm backward of n = Y_{n_a} (or act(a))          d_ln_gamma, d_ln_beta: per-CTA partials, fixed-order sum
+//   dU_k = dY_k act'(U_k), dK_k = Y_{k-1}^T . dU_k (TN GEMM), dY_{k-1} = dU_k . K_k^T;  d_a = dY_0 / div(v), rows >= Vt zero
+//   dQ[u, l] = sum_{(u->v) in A_l} d_a[v]   (reverse index)
+//   dZ_{n_e} = dQ act'(P), dE_{l,j} = A_{j-1}[:, l]^T . dZ_j[:, l] (A_0 = h), dZ_{j-1}[:, l] = (dZ_j[:, l] . E_{l,j}^T) act'(Z_{j-1})
+//   d_h = dZ_1 . [E_{0,1}|..|E_{L-1,1}]^T (V rows);  edge MLP None: d_h = sum_l dQ[:, l] in l order
+// The per-type transposed product dZ_j[:, l] . E_{l,j}^T is one BATCH_K_BLOCKS_T launch per type (see DESIGN.md 5.4f).
+extern "C" int rgnn_rgin_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d_in, int32_t d_out,
+                                  const float* const* edge_mlp_kernels, const int32_t* edge_mlp_dims,
+                                  int num_edge_mlp_hidden_layers, const float* const* aggr_kernels, const int32_t* aggr_dims,
+                                  int num_aggr_mlp_hidden_layers, const float* ln_gamma, const float* ln_beta, int activation,
+                                  int aggregation, int use_target, const float* grad_out, float* grad_h,
+                                  float* const* grad_edge_mlp_kernels, float* const* grad_aggr_kernels, float* grad_ln_gamma,
+                                  float* grad_ln_beta, void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  rgnn_plan* plan = const_cast<rgnn_plan*>(plan_c);   // the reverse index is built lazily inside the plan
+  RGNN_REQUIRE(plan != nullptr, "rgin_backward: plan is NULL");
+  RGNN_REQUIRE(h != nullptr, "rgin_backward: node_embeddings is NULL");
+  RGNN_REQUIRE(ln_gamma != nullptr, "rgin_backward: ln_gamma is NULL");
+  RGNN_REQUIRE(ln_beta != nullptr, "rgin_backward: ln_beta is NULL");
+  RGNN_REQUIRE(grad_out != nullptr, "rgin_backward: grad_out is NULL");
+  RGNN_REQUIRE(d_in > 0 && d_out > 0 && (d_in % 4) == 0 && (d_out % 4) == 0,
+               "rgin_backward: d_in / d_out must be positive multiples of 4 (d_in=%d, d_out=%d)", d_in, d_out);
+  if (use_target) {
+    set_error("rgin_backward: use_target_state_as_input = 1 (target-conditioned messages) is not implemented in this build");
+    return RGNN_E_UNSUPPORTED;
+  }
+  if (d_out > RGNN_MAX_STATE_DIM) {
+    set_error("rgin_backward: d_out %d > %d (the layer norm holds a row per warp) is not supported", d_out, RGNN_MAX_STATE_DIM);
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_PROPAGATE(check_act(activation, "rgin_backward"));
+  RGNN_PROPAGATE(check_agg(aggregation, "rgin_backward"));
+  if (aggregation == RGNN_AGG_MAX) {
+    set_error("rgin_backward: the gradient of 'max' aggregation is not implemented in this build");
+    return RGNN_E_UNSUPPORTED;
+  }
+  const int n_e = num_edge_mlp_hidden_layers < 0 ? 0 : num_edge_mlp_hidden_layers + 1;
+  const int n_a = num_aggr_mlp_hidden_layers < 0 ? 0 : num_aggr_mlp_hidden_layers + 1;
+  RGNN_REQUIRE(n_e <= RGNN_MAX_MLP_LAYERS, "rgin_backward: edge MLP with %d layers exceeds the supported %d", n_e, RGNN_MAX_MLP_LAYERS);
+  RGNN_REQUIRE(n_a <= RGNN_MAX_MLP_LAYERS, "rgin_backward: aggregation MLP with %d layers exceeds the supported %d", n_a,
+               RGNN_MAX_MLP_LAYERS);
+  const int V = plan->V, Vt = plan->Vt, L = plan->L, D = d_out;
+  const int32_t* ed = edge_mlp_dims;
+  const int32_t* ad = aggr_dims;
+  if (n_e > 0) {
+    RGNN_REQUIRE(edge_mlp_kernels != nullptr, "rgin_backward: edge_mlp_kernels is NULL");
+    RGNN_REQUIRE(ed != nullptr, "rgin_backward: edge_mlp_dims is NULL");
+    RGNN_REQUIRE(ed[0] == d_in, "rgin_backward: edge_mlp_dims[0] = %d does not match d_in %d", ed[0], d_in);
+    for (int j = 1; j <= n_e; ++j)
+      RGNN_REQUIRE(ed[j] > 0 && (ed[j] % 4) == 0, "rgin_backward: edge_mlp_dims[%d] = %d must be a positive multiple of 4", j, ed[j]);
+    RGNN_PROPAGATE(check_mlp_widths(ed, n_e, d_in, d_out, "edge MLP", "rgin_backward"));
+    for (int i = 0; i < L * n_e; ++i) RGNN_REQUIRE(edge_mlp_kernels[i] != nullptr, "rgin_backward: edge MLP kernel %d is NULL", i);
+  }
+  const int width = n_e > 0 ? ed[n_e] : d_in;   // message width
+  if (n_a > 0) {
+    RGNN_REQUIRE(aggr_kernels != nullptr, "rgin_backward: aggr_kernels is NULL");
+    RGNN_REQUIRE(ad != nullptr, "rgin_backward: aggr_dims is NULL");
+    RGNN_REQUIRE(ad[0] == width && ad[n_a] == D, "rgin_backward: aggr_dims [%d .. %d] do not match [%d .. %d]", ad[0], ad[n_a], width, D);
+    for (int k = 1; k <= n_a; ++k)
+      RGNN_REQUIRE(ad[k] > 0 && (ad[k] % 4) == 0, "rgin_backward: aggr_dims[%d] = %d must be a positive multiple of 4", k, ad[k]);
+    RGNN_PROPAGATE(check_mlp_widths(ad, n_a, d_in, d_out, "aggregation MLP", "rgin_backward"));
+    for (int k = 0; k < n_a; ++k) RGNN_REQUIRE(aggr_kernels[k] != nullptr, "rgin_backward: aggregation MLP kernel %d is NULL", k);
+  } else {
+    RGNN_REQUIRE(width == D, "rgin_backward: message width %d != d_out %d and no aggregation MLP maps it", width, D);
+  }
+  RGNN_REQUIRE(aligned16(h) && aligned16(grad_out) && aligned16(ln_gamma) && aligned16(ln_beta),
+               "rgin_backward: node_embeddings / grad_out / ln_gamma / ln_beta must be 16-byte aligned");
+  RGNN_REQUIRE(aligned16(grad_h) && aligned16(grad_ln_gamma) && aligned16(grad_ln_beta),
+               "rgin_backward: grad_node_embeddings / grad_ln_gamma / grad_ln_beta must be 16-byte aligned");
+  RGNN_REQUIRE(grad_h == nullptr || (grad_h != h && grad_h != grad_out),
+               "rgin_backward: grad_node_embeddings must not alias node_embeddings or grad_out");
+  const bool want_e = grad_edge_mlp_kernels != nullptr && n_e > 0;
+  const bool want_a = grad_aggr_kernels != nullptr && n_a > 0;
+  if (want_e)
+    for (int i = 0; i < L * n_e; ++i)
+      RGNN_REQUIRE(grad_edge_mlp_kernels[i] != nullptr && aligned16(grad_edge_mlp_kernels[i]),
+                   "rgin_backward: grad edge MLP kernel %d is NULL / misaligned", i);
+  if (want_a)
+    for (int k = 0; k < n_a; ++k)
+      RGNN_REQUIRE(grad_aggr_kernels[k] != nullptr && aligned16(grad_aggr_kernels[k]),
+                   "rgin_backward: grad aggregation MLP kernel %d is NULL / misaligned", k);
+
+  // every carve-out and the largest weight-image scratch of the dense contractions, before anything is enqueued
+  Arena ar(workspace, workspace_bytes);
+  float* Z[RGNN_MAX_MLP_LAYERS + 1] = {};   // Z_j [V, L, ed[j]], then dZ_j in place
+  float* Aj[RGNN_MAX_MLP_LAYERS + 1] = {};  // act(Z_j), j < n_e
+  float* U[RGNN_MAX_MLP_LAYERS + 1] = {};   // U_k [Vt, ad[k]], then dU_k in place
+  float* Y[RGNN_MAX_MLP_LAYERS + 1] = {};   // Y_k = act(U_k) [Vt, ad[k]], then dY_k; Y_0 = a
+  int gw = width;                           // dQ, then each dA_{j-1}: [V, L, <= gw]
+  for (int j = 1; j <= n_e; ++j) Z[j] = ar.floats((size_t)V * L * ed[j]);
+  for (int j = 1; j < n_e; ++j) { Aj[j] = ar.floats((size_t)V * L * ed[j]); gw = std::max(gw, (int)ed[j]); }
+  float* G = ar.floats((size_t)V * L * gw);
+  float* a = ar.floats((size_t)V * width);   // the aggregate, then d_a (every row: the reverse gather reads any target)
+  Y[0] = a;
+  for (int k = 1; k <= n_a; ++k) U[k] = ar.floats((size_t)Vt * ad[k]);
+  for (int k = 1; k < n_a; ++k) Y[k] = ar.floats((size_t)Vt * ad[k]);
+  float* nrm = ar.floats((size_t)Vt * D);   // n, then dn in place
+  if (n_a > 0) Y[n_a] = nrm;
+  float* ln_part = ar.floats((size_t)film_ln_blocks(Vt) * 2 * D + 4);
+  float* tn_scratch = nullptr;
+  {
+    size_t n = 0;
+    if (want_e) {
+      n = gemm_tn_scratch_floats(d_in, L * ed[1], V);
+      for (int j = 2; j <= n_e; ++j) n = std::max(n, gemm_tn_scratch_floats(ed[j - 1], ed[j], V));
+    }
+    if (want_a)
+      for (int k = 1; k <= n_a; ++k) n = std::max(n, gemm_tn_scratch_floats(ad[k - 1], ad[k], Vt));
+    if (n > 0) tn_scratch = ar.floats(n);
+  }
+  SegParams heavy;
+  seg_heavy_scratch(heavy, plan, ar, width);
+
+  // the dense contractions
+  const float* bp[RGNN_MAX_EDGE_TYPES];
+  auto fwd_edge = [&](int j) {   // Z_j = A_{j-1} . E_{l,j} per type (j = 1: the shared-A GEMM on h)
+    GemmParams g;
+    g.M = V; g.N = ed[j]; g.C = Z[j]; g.ldc = L * ed[j]; g.ldb1 = ed[j]; g.batch = L;
+    if (j == 1) { g.A1 = h; g.lda1 = d_in; g.K1 = d_in; g.batch_mode = BATCH_SHARED_A; }
+    else { g.A1 = Aj[j - 1]; g.lda1 = L * ed[j - 1]; g.K1 = ed[j - 1]; g.batch_mode = BATCH_COL_BLOCKS; }
+    for (int l = 0; l < L; ++l) { g.bptr[l] = edge_mlp_kernels[l * n_e + j - 1]; g.bptr2[l] = nullptr; }
+    return g;
+  };
+  auto bwd_edge = [&](int j, int l) {   // dA_{j-1}[:, l] = dZ_j[:, l] . E_{l,j}^T  (j >= 2)
+    GemmParams g;
+    g.A1 = Z[j] + (size_t)l * ed[j]; g.lda1 = L * ed[j]; g.K1 = ed[j]; g.M = V; g.N = ed[j - 1];
+    g.C = G + (size_t)l * ed[j - 1]; g.ldc = L * ed[j - 1]; g.ldb1 = ed[j];
+    g.batch_mode = BATCH_K_BLOCKS_T; g.batch = 1; g.k_block = ed[j]; g.bptr[0] = edge_mlp_kernels[l * n_e + j - 1]; g.bptr2[0] = nullptr;
+    return g;
+  };
+  auto fwd_aggr = [&](int k) {   // U_k = Y_{k-1} . K_k
+    GemmParams g;
+    g.A1 = Y[k - 1]; g.lda1 = ad[k - 1]; g.K1 = ad[k - 1]; g.B1 = aggr_kernels[k - 1]; g.ldb1 = ad[k];
+    g.M = Vt; g.N = ad[k]; g.C = U[k]; g.ldc = ad[k];
+    return g;
+  };
+  auto bwd_aggr = [&](int k) {   // dY_{k-1} = dU_k . K_k^T
+    GemmParams g;
+    g.A1 = U[k]; g.lda1 = ad[k]; g.K1 = ad[k]; g.M = Vt; g.N = ad[k - 1]; g.C = Y[k - 1]; g.ldc = ad[k - 1]; g.ldb1 = ad[k];
+    g.batch_mode = BATCH_K_BLOCKS_T; g.batch = 1; g.k_block = ad[k]; g.bptr[0] = aggr_kernels[k - 1]; g.bptr2[0] = nullptr;
+    return g;
+  };
+  GemmParams gH;   // d_h = dZ_1 . [E_{0,1}|..|E_{L-1,1}]^T
+  if (n_e > 0) {
+    gH.A1 = Z[1]; gH.lda1 = L * ed[1]; gH.K1 = L * ed[1]; gH.M = V; gH.N = d_in; gH.C = grad_h; gH.ldc = d_in; gH.ldb1 = ed[1];
+    gH.batch_mode = BATCH_K_BLOCKS_T; gH.batch = L; gH.k_block = ed[1];
+    for (int l = 0; l < L; ++l) { gH.bptr[l] = edge_mlp_kernels[l * n_e]; gH.bptr2[l] = nullptr; }
+  }
+  size_t pack = 0;
+  if (V > 0) {
+    for (int j = 1; j <= n_e; ++j) pack = std::max(pack, gemm_tc_pack_bytes(fwd_edge(j)));
+    for (int j = 2; j <= n_e; ++j)
+      for (int l = 0; l < L; ++l) pack = std::max(pack, gemm_tc_pack_bytes(bwd_edge(j, l)));
+    if (grad_h != nullptr && n_e > 0) pack = std::max(pack, gemm_tc_pack_bytes(gH));
+  }
+  if (Vt > 0)
+    for (int k = 1; k <= n_a; ++k) pack = std::max(pack, std::max(gemm_tc_pack_bytes(fwd_aggr(k)), gemm_tc_pack_bytes(bwd_aggr(k))));
+  {
+    const size_t mark = ar.used;
+    ar.floats(pack / sizeof(float));
+    RGNN_PROPAGATE(check_ws(ar, "rgin_backward"));
+    ar.used = mark;
+  }
+  RGNN_PROPAGATE(plan_ensure_reverse(plan, stream));
+  RGNN_PROPAGATE(plan_wait_sources(plan, stream));   // the edge MLP reads the halo rows
+
+  // forward: the edge MLP on the node rows, the aggregate, the aggregation MLP
+  for (int j = 1; j <= n_e; ++j) {
+    if (V > 0) RGNN_PROPAGATE(run_gemm(fwd_edge(j), ar, stream));
+    if (j < n_e) RGNN_PROPAGATE(launch_rgin_act(Z[j], (long)V * L * ed[j], activation, Aj[j], stream));
+  }
+  {
+    SegParams s;
+    seg_from_plan(s, plan);
+    s.D = width;
+    if (n_e > 0) { s.table = Z[n_e]; s.stride_idx = (long)L * width; s.stride_type = width; s.act_msg = activation; }   // :128-129
+    else { s.table = h; s.stride_idx = d_in; s.stride_type = 0; }
+    s.agg = aggregation; s.out = a; s.ld_out = width; s.heavy_scratch = heavy.heavy_scratch;
+    RGNN_PROPAGATE(launch_seg_reduce(s, stream));
+  }
+  for (int k = 1; k <= n_a; ++k) {
+    if (Vt > 0) RGNN_PROPAGATE(run_gemm(fwd_aggr(k), ar, stream));
+    RGNN_PROPAGATE(launch_rgin_act(U[k], (long)Vt * ad[k], activation, Y[k], stream));
+  }
+  if (n_a == 0) RGNN_PROPAGATE(launch_rgin_act(a, (long)Vt * D, activation, nrm, stream));   // :138
+
+  // layer norm, then the aggregation MLP down to d_a
+  FilmLnBwdParams lp;
+  lp.rows = Vt; lp.D = D; lp.agg = RGNN_AGG_SUM; lp.seg_off = plan->seg_off; lp.grad_out = grad_out; lp.ln_gamma = ln_gamma;
+  lp.a = nrm; lp.partial = ln_part;
+  RGNN_PROPAGATE(launch_film_ln_backward(lp, stream));
+  RginGradParams gp;
+  gp.act = activation;
+  if (n_a == 0) {
+    gp.rows = V; gp.valid = Vt; gp.width = width; gp.agg = aggregation; gp.seg_off = plan->seg_off;
+    gp.g = nrm; gp.x = a; gp.out = a;
+    RGNN_PROPAGATE(launch_rgin_act_grad(gp, stream));
+  } else {
+    gp.rows = gp.valid = Vt; gp.width = D; gp.g = nrm; gp.x = U[n_a]; gp.out = U[n_a];
+    RGNN_PROPAGATE(launch_rgin_act_grad(gp, stream));
+    for (int k = n_a; k >= 1; --k) {
+      if (want_a) {
+        GemmTnOut tn;
+        tn.block_cols = ad[k]; tn.ld = ad[k]; tn.ptr[0] = grad_aggr_kernels[k - 1];
+        RGNN_PROPAGATE(launch_gemm_tn(Y[k - 1], ad[k - 1], U[k], ad[k], ad[k - 1], ad[k], Vt, tn, tn_scratch, stream));
+      }
+      if (Vt > 0) RGNN_PROPAGATE(run_gemm(bwd_aggr(k), ar, stream));   // dY_{k-1} overwrites Y_{k-1} after d_K_k read it
+      if (k > 1) {
+        gp.rows = gp.valid = Vt; gp.width = ad[k - 1]; gp.g = Y[k - 1]; gp.x = U[k - 1]; gp.out = U[k - 1];
+        RGNN_PROPAGATE(launch_rgin_act_grad(gp, stream));
+      }
+    }
+    gp.rows = V; gp.valid = Vt; gp.width = width; gp.act = RGNN_ACT_LINEAR; gp.agg = aggregation; gp.seg_off = plan->seg_off;
+    gp.g = a; gp.x = nullptr; gp.out = a;
+    RGNN_PROPAGATE(launch_rgin_act_grad(gp, stream));
+  }
+
+  // the source side: dQ[u, l] = sum over the edges (u -> v) of type l of d_a[v]; every (u, l) row is written
+  {
+    SegParams r;   // reverse index: segment = (source u, type l); gathered row = d_a[original target]
+    r.V = V * L; r.L = L; r.D = width;
+    r.seg_off = plan->rev_seg_off; r.e_idx = plan->rev_src; r.e_type = plan->rev_type;
+    r.table = a; r.stride_idx = width; r.stride_type = 0;
+    r.heavy_list = plan->rev_heavy_list; r.heavy_count = plan->err_flag + 2;
+    r.heavy_threshold = RGNN_HEAVY_SEGMENT; r.heavy_known = -1;
+    r.agg = RGNN_AGG_SUM; r.out = G; r.ld_out = width;
+    RGNN_PROPAGATE(launch_seg_reduce(r, stream));
+  }
+
+  // the edge MLP, from the message down to h
+  if (n_e == 0) {
+    if (grad_h != nullptr) RGNN_PROPAGATE(launch_rgin_type_sum(G, V, L, d_in, grad_h, stream));
+  } else {
+    gp = RginGradParams();
+    gp.act = activation; gp.rows = gp.valid = V; gp.width = L * width; gp.g = G; gp.x = Z[n_e]; gp.out = Z[n_e];
+    RGNN_PROPAGATE(launch_rgin_act_grad(gp, stream));
+    for (int j = n_e; j >= 2; --j) {
+      if (want_e)
+        for (int l = 0; l < L; ++l) {
+          GemmTnOut tn;
+          tn.block_cols = ed[j]; tn.ld = ed[j]; tn.ptr[0] = grad_edge_mlp_kernels[l * n_e + j - 1];
+          RGNN_PROPAGATE(launch_gemm_tn(Aj[j - 1] + (size_t)l * ed[j - 1], L * ed[j - 1], Z[j] + (size_t)l * ed[j], L * ed[j],
+                                        ed[j - 1], ed[j], V, tn, tn_scratch, stream));
+        }
+      if (V > 0)
+        for (int l = 0; l < L; ++l) RGNN_PROPAGATE(run_gemm(bwd_edge(j, l), ar, stream));
+      gp.width = L * ed[j - 1]; gp.g = G; gp.x = Z[j - 1]; gp.out = Z[j - 1];
+      RGNN_PROPAGATE(launch_rgin_act_grad(gp, stream));
+    }
+    if (want_e) {
+      GemmTnOut tn;
+      tn.block_cols = ed[1]; tn.ld = ed[1];
+      for (int l = 0; l < L; ++l) tn.ptr[l] = grad_edge_mlp_kernels[l * n_e];
+      RGNN_PROPAGATE(launch_gemm_tn(h, d_in, Z[1], L * ed[1], d_in, L * ed[1], V, tn, tn_scratch, stream));
+    }
+    if (grad_h != nullptr && V > 0) RGNN_PROPAGATE(run_gemm(gH, ar, stream));
+  }
+  if (grad_ln_gamma != nullptr || grad_ln_beta != nullptr)
+    RGNN_PROPAGATE(launch_film_ln_param_reduce(ln_part, Vt, D, grad_ln_gamma, grad_ln_beta, stream));
   return RGNN_OK;
 }
 

@@ -207,4 +207,21 @@ inline int ggnn_colsum_blocks(int rows) {
 }
 int launch_ggnn_bias_grad(const float* x, int rows, int N, float* partial, float* out, cudaStream_t stream);
 
+// ---- rgnn_rgin_backward (rgin_backward.cu) ----
+// y[0:n] = act(x[0:n])  (n % 4 == 0)
+int launch_rgin_act(const float* x, long n, int act, float* y, cudaStream_t stream);
+// out [rows, width]: rows < valid = g act'(x) (act LINEAR: g; x unread), divided by the mean / sqrt_n divisor of v when agg
+// asks for it (seg_off: all incoming edges of v); rows >= valid zero.  out may be g or x.
+struct RginGradParams {
+  long rows = 0, valid = 0;
+  int width = 0, act = RGNN_ACT_LINEAR, agg = RGNN_AGG_SUM;
+  const int32_t* seg_off = nullptr;
+  const float* g = nullptr;
+  const float* x = nullptr;
+  float* out = nullptr;
+};
+int launch_rgin_act_grad(const RginGradParams& p, cudaStream_t stream);
+// out [V, D] = sum over l in order of dq [V, L, D]
+int launch_rgin_type_sum(const float* dq, int V, int L, int D, float* out, cudaStream_t stream);
+
 }  // namespace rgnn

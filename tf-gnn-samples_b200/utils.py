@@ -16,6 +16,7 @@ LAYER_RGCN, LAYER_GGNN, LAYER_RGAT, LAYER_FILM, LAYER_EDGE_MLP, LAYER_RGIN, LAYE
 LAYER_FILM_BACKWARD = 8   # rgnn_workspace_bytes of rgnn_film_backward
 LAYER_RGAT_BACKWARD = 9   # rgnn_workspace_bytes of rgnn_rgat_backward
 LAYER_GGNN_BACKWARD = 10  # rgnn_workspace_bytes of rgnn_ggnn_backward
+LAYER_RGIN_BACKWARD = 11  # rgnn_workspace_bytes of rgnn_rgin_backward
 
 _ACTIVATIONS = {"linear": ACT_LINEAR, "tanh": ACT_TANH, "relu": ACT_RELU, "leaky_relu": ACT_LEAKY_RELU,
                 "elu": ACT_ELU, "selu": ACT_SELU, "gelu": ACT_GELU}
