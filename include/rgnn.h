@@ -25,7 +25,7 @@
  *   capture   run eagerly once before capturing: every layer with the weight cache on (a cache miss
  *             during capture is an error), and the first backward on a plan (rgnn_rgcn_backward /
  *             rgnn_film_backward / rgnn_rgat_backward / rgnn_ggnn_backward / rgnn_rgin_backward /
- *             rgnn_edge_aggregate_backward build the plan's reverse index then; inside a capture they
+ *             rgnn_rgdcn_backward / rgnn_edge_aggregate_backward build the plan's reverse index then; inside a capture they
  *             return RGNN_E_INVALID).  A plan built with RGNN_PLAN_DEFERRED_CHECK inside a capture is
  *             filled only when the graph is replayed: call rgnn_plan_status after a replay.  A graph
  *             captured with the weight cache on reads the cached images: rgnn_weight_cache_clear (and
@@ -86,7 +86,8 @@ enum rgnn_layer_kind {
   RGNN_LAYER_EDGE_MLP = 4, RGNN_LAYER_RGIN = 5, RGNN_LAYER_RGCN_BACKWARD = 6,
   RGNN_LAYER_RGDCN = 7,  /* rgnn_workspace_bytes: pass channel_dim as mlp_layers */
   RGNN_LAYER_FILM_BACKWARD = 8, RGNN_LAYER_RGAT_BACKWARD = 9, RGNN_LAYER_GGNN_BACKWARD = 10,
-  RGNN_LAYER_RGIN_BACKWARD = 11
+  RGNN_LAYER_RGIN_BACKWARD = 11,
+  RGNN_LAYER_RGDCN_BACKWARD = 12  /* rgnn_workspace_bytes: pass channel_dim as mlp_layers */
 };
 
 typedef struct rgnn_plan rgnn_plan_t;
@@ -349,6 +350,37 @@ RGNN_API int rgnn_rgdcn_forward(const rgnn_plan_t* plan, const float* h, int32_t
                        const float* const* channel_weights, int use_full_state, const float* num_incoming,
                        int activation, int aggregation, int normalize, int num_timesteps, float* out,
                        void* workspace, size_t workspace_bytes, void* stream);
+
+/* Backward of ONE timestep of sparse_rgdcn_layer (rgdcn.py:116-165; all four variants, sum / mean / sqrt_n, every
+ * activation): the gradients TensorFlow autodiff produces.  Gradients are written, not accumulated.  No forward state is
+ * needed: the call recomputes the dynamic kernels' pre-activations and the aggregate from its inputs, and builds no
+ * per-edge tensor.
+ *   node_embeddings [V, d]: this timestep's INPUT; channel_weights, use_full_state, num_incoming, activation, aggregation,
+ *   normalize: as rgnn_rgdcn_forward (host array of L * num_channels kernels, type-major, [d or K, K*K] each)
+ *   grad_out [num_targets, d] (rows [0, num_targets) of the plan, rgnn_plan_set_num_targets)
+ *   grad_node_embeddings [V, d] covers EVERY local row (halo rows included: what rgnn_halo_exchange_backward consumes) or
+ *   NULL, and must not alias node_embeddings or grad_out
+ *   grad_channel_weights: host array of L * num_channels device pointers laid out like channel_weights, or NULL.
+ *   tie_channel_weights = 1 (one kernel per edge type, rgdcn.py:96,105-107): every entry of type l must be the same pointer,
+ *   in channel_weights and in grad_channel_weights, and dF_l (the sum over the channels) is written once.  Untied: the
+ *   entries of grad_channel_weights must be distinct.  Either violation is refused, naming the argument.
+ * Limits are the forward's: K = d / num_channels a power of two in [4, 128], num_channels <= RGNN_MAX_EDGE_TYPES, 16-byte
+ * alignment; d > RGNN_MAX_STATE_DIM and 'max' aggregation: RGNN_E_UNSUPPORTED.  Every argument is checked and the workspace
+ * sized before anything is enqueued.  The first backward on a plan builds its reverse index (as rgnn_rgcn_backward; not
+ * inside a capture).  Two identical calls are bit-identical (no atomics: every output has one writer, every sum a fixed
+ * order).
+ * Several timesteps are the caller's loop: run the forward with num_timesteps = 1 per timestep keeping each input, call
+ * this from the last timestep down (grad_out of step t = grad_node_embeddings of step t + 1), and add the shared weights'
+ * gradients of the steps.
+ * Workspace: rgnn_workspace_bytes(plan, RGNN_LAYER_RGDCN_BACKWARD, d, d, K): with V = num_nodes, Vt = num_targets,
+ * L = num_edge_types, C = d / K, Q = min(L C, 64) K^2,
+ * (Vt L d K + 2 V L d + Vt d + Vt L K^2 + d Q + 2 (Q + 128)(d + 128) + 2163712) floats plus the weight-image scratch of the
+ * forward's bound, 2 (4 d + 64)(4 L d + 4 d + 512) floats, plus 8192 bytes.  No term grows with the number of edges. */
+RGNN_API int rgnn_rgdcn_backward(const rgnn_plan_t* plan, const float* node_embeddings, int32_t d, int32_t num_channels,
+                        const float* const* channel_weights, int use_full_state, int tie_channel_weights,
+                        const float* num_incoming, int activation, int aggregation, int normalize,
+                        const float* grad_out, float* grad_node_embeddings, float* const* grad_channel_weights,
+                        void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- one large graph over several GPUs: node-range partition + halo exchange (SURVEY.md 8e) --------------------------
  * The reference is single-device; this is the multi-GPU form of ITS batch (tasks/varmisuse_task.py:451-538 packs up to

@@ -15,7 +15,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_DIR = os.path.join(PKG_DIR, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "librgnn.so")
 STAMP = os.path.join(LIB_DIR, "librgnn.stamp")
-SOURCES = ["gemm_wgmma.cu", "gemm_tn_wgmma.cu", "plan.cu", "halo.cu", "seg_kernels.cu", "film_backward.cu", "rgat_backward.cu", "ggnn_backward.cu", "rgin_backward.cu", "layers.cu", "batch.cu"]
+SOURCES = ["gemm_wgmma.cu", "gemm_tn_wgmma.cu", "plan.cu", "halo.cu", "seg_kernels.cu", "film_backward.cu", "rgat_backward.cu", "ggnn_backward.cu", "rgin_backward.cu", "rgdcn_backward.cu", "layers.cu", "batch.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 

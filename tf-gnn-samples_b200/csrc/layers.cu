@@ -9,6 +9,8 @@
 #include <algorithm>
 #include <mutex>
 #include <atomic>
+#include <utility>
+#include <vector>
 #include <string.h>
 #include <stdlib.h>
 
@@ -351,6 +353,15 @@ extern "C" size_t rgnn_workspace_bytes(const rgnn_plan_t* plan, int layer_kind, 
                + (RGNN_WAVE_SMS * 16384 + L * dm * dm) + 64 * 1024;                             // split-K tiles of d_E / d_K
       break;
     }
+    case RGNN_LAYER_RGDCN_BACKWARD: {   // mlp_layers carries channel_dim K; P / dP [Vt, L, d K]; dS, dQ [V, L, d];
+      const size_t Vt = (size_t)plan->Vt, dd = (size_t)d_out, Kc = (size_t)(mlp_layers > 0 ? mlp_layers : 16), KK = Kc * Kc;
+      const size_t C = dd / Kc > 0 ? dd / Kc : 1, Q = std::min(L * C, (size_t)RGNN_MAX_EDGE_TYPES) * KK;   // d_h term [Vt, d];
+      floats = Vt * L * dd * Kc + 2 * V * L * dd + Vt * dd + Vt * L * KK   // dP summed over channels [Vt, L, K K];
+               + (RGNN_WAVE_SMS * 16384 + dd * Q)                         // split-K tiles of dF;
+               + 2 * (Q + 128) * (dd + 128) + 1024;                       // weight images of the largest GEMM
+      const size_t fwd_pack = 2 * (2 * dm + 64) * (2 * L * dm + 2 * dm + 512);
+      return (floats + fwd_pack) * sizeof(float) + pad;   // no heavy-target scratch: nothing sized by M
+    }
     default: return 0;
   }
   // scratch for the pre-swizzled hi/lo weight images of the largest dense contraction of the layer
@@ -569,6 +580,208 @@ extern "C" int rgnn_rgdcn_forward(const rgnn_plan_t* plan, const float* h, int32
     r.agg = aggregation; r.act_out = activation; r.out = dst;
     RGNN_PROPAGATE(launch_rgdcn_edges(r, stream));
     cur = dst;
+  }
+  return RGNN_OK;
+}
+
+// Backward of ONE timestep of sparse_rgdcn_layer (sum / mean / sqrt_n): what tf.gradients produces for gnns/rgdcn.py:116-165.
+// No forward state is kept and nothing per edge is built (rgdcn_backward.cu has the math of the edge kernel):
+//   P = x . F_{l,c} (wgmma GEMM, no activation: the Vt wanted target rows)
+//   per target: a, delta, dS [V, L, D] (rows >= Vt zero) and dP over P                     (rgdcn_bwd_target_kernel)
+//   d_h = sum_l (sum_{(u->v) in A_l} dS[v, l])  (reverse-index segment reduce, then the types in order)
+//         + dP . F^T on the Vt target rows (transposed-image GEMM)
+//   dF_{l,c} = x^T . dP[:, l, c] (split-K TN GEMM; tied: one dF_l = sum over c)
+// Layout of P: full state keeps the forward's [Vt, L, C, K*K], so the d_h term is a BATCH_K_BLOCKS_T GEMM over the L C
+// kernels and dF one TN GEMM with a K*K column block per kernel (both in chunks of RGNN_MAX_EDGE_TYPES kernels).  Per channel
+// it is [Vt, C, L, K*K]: the L kernels of a channel are adjacent, so d_h[:, c] is a BATCH_K_BLOCKS_T GEMM per channel, dF of
+// channel c one TN GEMM over h[:, c], and the tied dF_l one TN GEMM over h viewed as [Vt C, K] rows.  The d_h GEMMs contract
+// at most 1,024 columns of dP per launch (see below).
+extern "C" int rgnn_rgdcn_backward(const rgnn_plan_t* plan_c, const float* h, int32_t d, int32_t num_channels,
+                                   const float* const* channel_weights, int use_full_state, int tie_channel_weights,
+                                   const float* num_incoming, int activation, int aggregation, int normalize,
+                                   const float* grad_out, float* grad_h, float* const* grad_channel_weights,
+                                   void* workspace, size_t workspace_bytes, void* stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  rgnn_plan* plan = const_cast<rgnn_plan*>(plan_c);   // the reverse index is built lazily inside the plan
+  RGNN_REQUIRE(plan != nullptr, "rgdcn_backward: plan is NULL");
+  RGNN_REQUIRE(h != nullptr, "rgdcn_backward: node_embeddings is NULL");
+  RGNN_REQUIRE(grad_out != nullptr, "rgdcn_backward: grad_out is NULL");
+  RGNN_REQUIRE(channel_weights != nullptr, "rgdcn_backward: channel_weights is NULL");
+  RGNN_REQUIRE(d > 0 && (d % 4) == 0, "rgdcn_backward: the state dim d = %d must be a positive multiple of 4", d);
+  if (d > RGNN_MAX_STATE_DIM) {
+    set_error("rgdcn_backward: the state dim d = %d > %d is not supported in this build", d, RGNN_MAX_STATE_DIM);
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_PROPAGATE(check_act(activation, "rgdcn_backward"));
+  RGNN_PROPAGATE(check_agg(aggregation, "rgdcn_backward"));
+  if (aggregation == RGNN_AGG_MAX) {
+    set_error("rgdcn_backward: the gradient of 'max' aggregation is not implemented in this build");
+    return RGNN_E_UNSUPPORTED;
+  }
+  RGNN_REQUIRE(num_channels >= 1 && num_channels <= RGNN_MAX_EDGE_TYPES && (d % num_channels) == 0,
+               "rgdcn_backward: num_channels %d must divide the state dim %d (and be <= %d)", num_channels, d, RGNN_MAX_EDGE_TYPES);
+  const int V = plan->V, Vt = plan->Vt, L = plan->L, C = num_channels, K = d / num_channels, KK = K * K, LC = L * C;
+  const bool full = use_full_state != 0, tied = tie_channel_weights != 0;
+  RGNN_REQUIRE(K >= 4 && (K & (K - 1)) == 0 && K <= 128, "rgdcn_backward: channel_dim %d must be a power of two in [4, 128]", K);
+  RGNN_REQUIRE(!normalize || num_incoming != nullptr, "rgdcn_backward: normalize_by_num_incoming needs num_incoming");
+  for (int i = 0; i < LC; ++i)
+    RGNN_REQUIRE(channel_weights[i] != nullptr && aligned16(channel_weights[i]), "rgdcn_backward: channel weight %d is NULL / misaligned", i);
+  if (tied)
+    for (int i = 0; i < LC; ++i)
+      RGNN_REQUIRE(channel_weights[i] == channel_weights[i - i % C],
+                   "rgdcn_backward: tie_channel_weights = 1 needs one kernel per edge type, but channel_weights[%d] != channel_weights[%d]",
+                   i, i - i % C);
+  RGNN_REQUIRE(aligned16(h) && aligned16(grad_out), "rgdcn_backward: node_embeddings / grad_out must be 16-byte aligned");
+  RGNN_REQUIRE(aligned16(grad_h), "rgdcn_backward: grad_node_embeddings must be 16-byte aligned");
+  RGNN_REQUIRE(grad_h == nullptr || (grad_h != h && grad_h != grad_out),
+               "rgdcn_backward: grad_node_embeddings must not alias node_embeddings or grad_out");
+  float* const* gw = grad_channel_weights;
+  if (gw != nullptr) {
+    for (int i = 0; i < LC; ++i)
+      RGNN_REQUIRE(gw[i] != nullptr && aligned16(gw[i]), "rgdcn_backward: grad channel weight %d is NULL / misaligned", i);
+    std::pair<float*, int> seen[RGNN_MAX_EDGE_TYPES * RGNN_MAX_EDGE_TYPES];   // the distinct kernels' gradients
+    int n = 0;
+    for (int i = 0; i < LC; ++i) {
+      if (tied && i % C != 0) {
+        RGNN_REQUIRE(gw[i] == gw[i - i % C],
+                     "rgdcn_backward: tie_channel_weights = 1 needs one gradient per edge type, but grad_channel_weights[%d] != grad_channel_weights[%d]",
+                     i, i - i % C);
+        continue;
+      }
+      seen[n++] = {gw[i], i};
+    }
+    std::sort(seen, seen + n);
+    for (int i = 1; i < n; ++i)
+      RGNN_REQUIRE(seen[i].first != seen[i - 1].first, "rgdcn_backward: grad_channel_weights[%d] and grad_channel_weights[%d] alias",
+                   std::min(seen[i - 1].second, seen[i].second), std::max(seen[i - 1].second, seen[i].second));
+  }
+
+  // the P recompute: launch i is chunk i of RGNN_MAX_EDGE_TYPES kernels (full state) or channel i
+  const int n_dense = full ? (LC + RGNN_MAX_EDGE_TYPES - 1) / RGNN_MAX_EDGE_TYPES : C;
+  Arena ar(workspace, workspace_bytes);
+  float* P = ar.floats((size_t)Vt * LC * KK);
+  float* dS = ar.floats((size_t)V * L * d);
+  float* dQ = grad_h != nullptr ? ar.floats((size_t)V * L * d) : nullptr;
+  float* kin = grad_h != nullptr ? ar.floats((size_t)Vt * d) : nullptr;   // the kernel-input term of d_h
+  float* psum = (gw != nullptr && full && tied) ? ar.floats((size_t)Vt * L * KK) : nullptr;
+  auto chunk = [&](int i, int& z0, int& nz) { z0 = i * RGNN_MAX_EDGE_TYPES; nz = std::min(RGNN_MAX_EDGE_TYPES, LC - z0); };
+  auto fwd_p = [&](int i) {   // P = x . F (no activation)
+    GemmParams g;
+    g.M = Vt; g.N = KK; g.ldb1 = KK; g.batch_mode = BATCH_SHARED_A;
+    if (full) {
+      int z0, nz;
+      chunk(i, z0, nz);
+      g.A1 = h; g.lda1 = d; g.K1 = d; g.batch = nz; g.C = P + (size_t)z0 * KK; g.ldc = LC * KK;
+      for (int z = 0; z < nz; ++z) { g.bptr[z] = channel_weights[z0 + z]; g.bptr2[z] = nullptr; }
+    } else {
+      g.A1 = h + (size_t)i * K; g.lda1 = d; g.K1 = K; g.batch = L; g.C = P + (size_t)i * L * KK; g.ldc = LC * KK;
+      for (int l = 0; l < L; ++l) { g.bptr[l] = channel_weights[l * C + i]; g.bptr2[l] = nullptr; }
+    }
+    return g;
+  };
+  // kin = dP . F^T, contracted piece by piece: the tensor cores' fp32 accumulation loses accuracy along a long contraction
+  // (L K^2 = 65,536 at K = 128 gave 1e-4 relative error in one launch), so each launch contracts at most
+  // RGDCN_BWD_MAX_CHAIN columns of dP and the pieces are added into d_h in order.  A piece is the whole blocks z0 .. z0 + nz - 1
+  // (kc = K*K) or the columns [j0, j0 + kc) of block z0 (nz = 1); a block is one kernel F_{l,c} (per channel: the L kernels
+  // of one channel, z = l).
+  constexpr int RGDCN_BWD_MAX_CHAIN = 1024;
+  struct Piece { int z0, nz, j0, kc; };
+  std::vector<Piece> pieces;
+  {
+    const int nblk = full ? LC : L;
+    if (KK <= RGDCN_BWD_MAX_CHAIN) {
+      const int per = std::min(RGDCN_BWD_MAX_CHAIN / KK, (int)RGNN_MAX_EDGE_TYPES);
+      for (int z0 = 0; z0 < nblk; z0 += per) pieces.push_back({z0, std::min(per, nblk - z0), 0, KK});
+    } else {
+      for (int z = 0; z < nblk; ++z)
+        for (int j0 = 0; j0 < KK; j0 += RGDCN_BWD_MAX_CHAIN) pieces.push_back({z, 1, j0, RGDCN_BWD_MAX_CHAIN});
+    }
+  }
+  auto bwd_h = [&](const Piece& pc, int c) {   // full state: c unused
+    GemmParams g;
+    g.M = Vt; g.ldb1 = KK; g.k_block = pc.kc; g.K1 = pc.nz * pc.kc; g.batch = pc.nz; g.batch_mode = BATCH_K_BLOCKS_T;
+    g.lda1 = LC * KK; g.ldc = d;
+    if (full) {
+      g.A1 = P + (size_t)pc.z0 * KK + pc.j0; g.N = d; g.C = kin;
+      for (int z = 0; z < pc.nz; ++z) { g.bptr[z] = channel_weights[pc.z0 + z] + pc.j0; g.bptr2[z] = nullptr; }
+    } else {
+      g.A1 = P + ((size_t)c * L + pc.z0) * KK + pc.j0; g.N = K; g.C = kin + (size_t)c * K;
+      for (int z = 0; z < pc.nz; ++z) { g.bptr[z] = channel_weights[(pc.z0 + z) * C + c] + pc.j0; g.bptr2[z] = nullptr; }
+    }
+    return g;
+  };
+  float* tn_scratch = nullptr;
+  if (gw != nullptr) {
+    size_t n = 0;
+    if (full && tied) n = gemm_tn_scratch_floats(d, L * KK, Vt);
+    else if (full) for (int i = 0; i < n_dense; ++i) { int z0, nz; chunk(i, z0, nz); n = std::max(n, gemm_tn_scratch_floats(d, nz * KK, Vt)); }
+    else n = gemm_tn_scratch_floats(K, L * KK, tied ? Vt * C : Vt);
+    tn_scratch = ar.floats(n);
+  }
+  size_t pack = 0;
+  if (Vt > 0)
+    for (int i = 0; i < n_dense; ++i) pack = std::max(pack, gemm_tc_pack_bytes(fwd_p(i)));
+  if (Vt > 0 && grad_h != nullptr)
+    for (const Piece& pc : pieces)
+      for (int c = 0; c < (full ? 1 : C); ++c) pack = std::max(pack, gemm_tc_pack_bytes(bwd_h(pc, c)));
+  {
+    const size_t mark = ar.used;
+    ar.floats(pack / sizeof(float));
+    RGNN_PROPAGATE(check_ws(ar, "rgdcn_backward"));
+    ar.used = mark;
+  }
+  RGNN_PROPAGATE(plan_ensure_reverse(plan, stream));
+  RGNN_PROPAGATE(plan_wait_sources(plan, stream));   // the edge kernel gathers halo source rows
+
+  if (Vt > 0)
+    for (int i = 0; i < n_dense; ++i) RGNN_PROPAGATE(run_gemm(fwd_p(i), ar, stream));
+  RgdcnBwdParams r;
+  r.V = V; r.Vt = Vt; r.L = L; r.D = d; r.K = K; r.C = C; r.act = activation; r.agg = aggregation;
+  r.st_type = full ? C : 1; r.st_chan = full ? 1 : L;
+  r.seg_off = plan->seg_off; r.e_src = plan->e_src; r.e_type = plan->e_type;
+  r.h = h; r.grad_out = grad_out; r.num_incoming = normalize ? num_incoming : nullptr; r.scale_ld = V;
+  r.P = P; r.dS = dS;
+  RGNN_PROPAGATE(launch_rgdcn_bwd_target(r, stream));
+
+  if (grad_h != nullptr) {
+    SegParams s;   // reverse index: segment = (source u, type l); gathered row = dS[original target, l]
+    s.V = V * L; s.L = L; s.D = d;
+    s.seg_off = plan->rev_seg_off; s.e_idx = plan->rev_src; s.e_type = plan->rev_type;
+    s.table = dS; s.stride_idx = (long)L * d; s.stride_type = d;
+    s.heavy_list = plan->rev_heavy_list; s.heavy_count = plan->err_flag + 2;
+    s.heavy_threshold = RGNN_HEAVY_SEGMENT; s.heavy_known = -1;
+    s.agg = RGNN_AGG_SUM; s.out = dQ; s.ld_out = d;
+    RGNN_PROPAGATE(launch_seg_reduce(s, stream));
+    RGNN_PROPAGATE(launch_rgin_type_sum(dQ, V, L, d, grad_h, stream));
+    if (Vt > 0)
+      for (const Piece& pc : pieces) {   // in order
+        for (int c = 0; c < (full ? 1 : C); ++c) RGNN_PROPAGATE(run_gemm(bwd_h(pc, c), ar, stream));
+        RGNN_PROPAGATE(launch_add_rows(grad_h, kin, (long)Vt * d, stream));
+      }
+  }
+  if (gw != nullptr) {
+    GemmTnOut tn;
+    tn.block_cols = KK; tn.ld = KK;
+    if (full && tied) {
+      RGNN_PROPAGATE(launch_rgdcn_chan_sum(P, (long)Vt * L, C, KK, psum, stream));
+      for (int l = 0; l < L; ++l) tn.ptr[l] = gw[l * C];
+      RGNN_PROPAGATE(launch_gemm_tn(h, d, psum, L * KK, d, L * KK, Vt, tn, tn_scratch, stream));
+    } else if (full) {
+      for (int i = 0; i < n_dense; ++i) {
+        int z0, nz;
+        chunk(i, z0, nz);
+        for (int z = 0; z < nz; ++z) tn.ptr[z] = gw[z0 + z];
+        RGNN_PROPAGATE(launch_gemm_tn(h, d, P + (size_t)z0 * KK, LC * KK, d, nz * KK, Vt, tn, tn_scratch, stream));
+      }
+    } else if (tied) {   // h as [Vt C, K] rows, dP as [Vt C, L K*K] rows
+      for (int l = 0; l < L; ++l) tn.ptr[l] = gw[l * C];
+      RGNN_PROPAGATE(launch_gemm_tn(h, K, P, L * KK, K, L * KK, Vt * C, tn, tn_scratch, stream));
+    } else {
+      for (int c = 0; c < C; ++c) {
+        for (int l = 0; l < L; ++l) tn.ptr[l] = gw[l * C + c];
+        RGNN_PROPAGATE(launch_gemm_tn(h + (size_t)c * K, d, P + (size_t)c * L * KK, LC * KK, K, L * KK, Vt, tn, tn_scratch, stream));
+      }
+    }
   }
   return RGNN_OK;
 }

@@ -224,4 +224,24 @@ int launch_rgin_act_grad(const RginGradParams& p, cudaStream_t stream);
 // out [V, D] = sum over l in order of dq [V, L, D]
 int launch_rgin_type_sum(const float* dq, int V, int L, int D, float* out, cudaStream_t stream);
 
+// ---- rgnn_rgdcn_backward (rgdcn_backward.cu) ----
+// One warp per target row v < V: rows < Vt write dS [V, L, D] and overwrite the pre-activations P with dP; rows >= Vt zero
+// their dS rows.  P holds L * C blocks of K * K floats per target; W[v, l, c] is block v * L * C + l * st_type + c * st_chan
+// (full state: the forward's [Vt, L, C, K, K], st_type = C, st_chan = 1; per channel: [Vt, C, L, K, K], st_type = 1,
+// st_chan = L).
+struct RgdcnBwdParams {
+  int V = 0, Vt = 0, L = 1, D = 0, K = 0, C = 1, act = RGNN_ACT_LINEAR, agg = RGNN_AGG_SUM;
+  int st_type = 1, st_chan = 1;
+  const int32_t* seg_off = nullptr; const int32_t* e_src = nullptr; const int32_t* e_type = nullptr;
+  const float* h = nullptr;            // [V, D]   this timestep's input
+  const float* grad_out = nullptr;     // [Vt, D]
+  const float* num_incoming = nullptr; // [L, scale_ld] or NULL
+  int scale_ld = 0;
+  float* P = nullptr;                  // [Vt, L * C, K * K]  pre-activations in, dP out
+  float* dS = nullptr;                 // [V, L, D]
+};
+int launch_rgdcn_bwd_target(const RgdcnBwdParams& p, cudaStream_t stream);
+// out [rows, KK] = sum over c in order of dp [rows, C, KK]
+int launch_rgdcn_chan_sum(const float* dp, long rows, int C, int KK, float* out, cudaStream_t stream);
+
 }  // namespace rgnn

@@ -69,6 +69,8 @@ SIGNATURES = {
                                    c_int, c_int, c_int, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, _PTR, c_size_t, _PTR]),
     "rgnn_rgdcn_forward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, c_int, _PTR, c_int, c_int, c_int, c_int, _PTR,
                                    _PTR, c_size_t, _PTR]),
+    "rgnn_rgdcn_backward": (c_int, [_PTR, _PTR, c_int32, c_int32, _PTR, c_int, c_int, _PTR, c_int, c_int, c_int, _PTR, _PTR,
+                                    _PTR, _PTR, c_size_t, _PTR]),
     "rgnn_plan_set_num_targets": (c_int, [_PTR, c_int32]),
     "rgnn_segment_aggregate": (c_int, [_PTR, _PTR, c_int32, c_int, _PTR, _PTR]),
     "rgnn_edge_aggregate_forward": (c_int, [_PTR, _PTR, c_int32, _PTR, c_int, _PTR, _PTR]),

@@ -17,6 +17,7 @@ LAYER_FILM_BACKWARD = 8   # rgnn_workspace_bytes of rgnn_film_backward
 LAYER_RGAT_BACKWARD = 9   # rgnn_workspace_bytes of rgnn_rgat_backward
 LAYER_GGNN_BACKWARD = 10  # rgnn_workspace_bytes of rgnn_ggnn_backward
 LAYER_RGIN_BACKWARD = 11  # rgnn_workspace_bytes of rgnn_rgin_backward
+LAYER_RGDCN_BACKWARD = 12  # rgnn_workspace_bytes of rgnn_rgdcn_backward (pass channel_dim as mlp_layers)
 
 _ACTIVATIONS = {"linear": ACT_LINEAR, "tanh": ACT_TANH, "relu": ACT_RELU, "leaky_relu": ACT_LEAKY_RELU,
                 "elu": ACT_ELU, "selu": ACT_SELU, "gelu": ACT_GELU}
